@@ -26,6 +26,11 @@ def lib():
         _lib.orc_dinf.argtypes = [_P, _P, _P, _I, _I, _F, _P, _P]
         _lib.orc_aread8.argtypes = [_P, _P, _P, _I, _I, C.c_int16, _F, _I, _I]
         _lib.orc_areadinf.argtypes = [_P, _P, _P, _I, _I, _F, _I, _I, _P, _P]
+        _lib.orc_flowpathextremeup.argtypes = [_P, _P, _P, _I, _I, C.c_int16, _I, _I]
+        _lib.orc_gridnet.argtypes = [_P, _P, _I, _P, _P, _P, _I, _I, C.c_int16, _P, _P]
+        _lib.orc_dinfdecayaccum.argtypes = [_P, _P, _P, _P, _I, _I, _F, _F, _I, _I, _P, _P]
+        _lib.orc_dinfconclimaccum.argtypes = [_P, _P, _P, _P, _P, _I, _I, _F, _F, _F, _F, _I, _P, _P]
+        _lib.orc_dinftranslimaccum.argtypes = [_P, _P, _P, _P, _P, _P, _P, _I, _I, _F, _F, _F, _F, _I, _P, _P]
     return _lib
 
 
@@ -105,3 +110,77 @@ def _areadinf(ang, nodata=-3.4028234663852886e38, weights=None, dx=30.0, dy=30.0
     dxc, dyc = _rows(dx, ny), _rows(dy, ny)
     assert lib().orc_areadinf(_p(ang), _p(w), _p(out), nx, ny, nodata, int(w is not None), int(contcheck), _p(dxc), _p(dyc)) == 0
     return out
+
+
+# ---- the sibling sweep tools, with the signatures of taudem_b200.api's *_grid functions.  dx / dy: scalars or per-row arrays;
+#      dxc / dyc (per-row arrays) take precedence, as in the api.
+MISSINGFLOAT = -3.4028234663852886e38
+
+
+def _sizes(dx, dy, dxc, dyc, ny):
+    return _rows(dx if dxc is None else dxc, ny), _rows(dy if dyc is None else dyc, ny)
+
+
+def _f32(a, shape):
+    a = np.ascontiguousarray(a, np.float32)
+    assert a.shape == shape
+    return a
+
+
+def d8flowpathextremeup(p, sa, usemax=True, nodata=-32768, contcheck=True, outlets=None):
+    p = np.ascontiguousarray(p, np.int16); ny, nx = p.shape
+    sa = _f32(sa, p.shape)
+    out = np.empty((ny, nx), np.float32)
+    with _Outlets(outlets):
+        assert lib().orc_flowpathextremeup(_p(p), _p(sa), _p(out), nx, ny, nodata, int(usemax), int(contcheck)) == 0
+    return out
+
+
+def gridnet(p, mask=None, thresh=0, dx=30.0, dy=30.0, nodata=-32768, outlets=None, dxc=None, dyc=None):
+    """(plen, tlen, gord)"""
+    p = np.ascontiguousarray(p, np.int16); ny, nx = p.shape
+    m = None if mask is None else np.ascontiguousarray(mask, np.int32)
+    dxc, dyc = _sizes(dx, dy, dxc, dyc, ny)
+    plen, tlen, gord = np.empty((ny, nx), np.float32), np.empty((ny, nx), np.float32), np.empty((ny, nx), np.int16)
+    with _Outlets(outlets):
+        assert lib().orc_gridnet(_p(p), _p(m), int(thresh), _p(plen), _p(tlen), _p(gord), nx, ny, nodata, _p(dxc), _p(dyc)) == 0
+    return plen, tlen, gord
+
+
+def dinfdecayaccum(ang, dm, weights=None, dx=30.0, dy=30.0, nodata=MISSINGFLOAT, dm_nodata=-9999.0, contcheck=True, outlets=None, dxc=None, dyc=None):
+    ang = np.ascontiguousarray(ang, np.float32); ny, nx = ang.shape
+    dm = _f32(dm, ang.shape)
+    w = None if weights is None else _f32(weights, ang.shape)
+    dxc, dyc = _sizes(dx, dy, dxc, dyc, ny)
+    out = np.empty((ny, nx), np.float32)
+    with _Outlets(outlets):
+        assert lib().orc_dinfdecayaccum(_p(ang), _p(dm), _p(w), _p(out), nx, ny, nodata, dm_nodata, int(w is not None), int(contcheck), _p(dxc), _p(dyc)) == 0
+    return out
+
+
+def dinfconclimaccum(ang, dm, q, dg, csol=1.0, dx=30.0, dy=30.0, nodata=MISSINGFLOAT, dm_nodata=-9999.0, q_nodata=-9999.0, contcheck=True, outlets=None,
+                     dxc=None, dyc=None):
+    ang = np.ascontiguousarray(ang, np.float32); ny, nx = ang.shape
+    dm, q = _f32(dm, ang.shape), _f32(q, ang.shape)
+    dg = np.ascontiguousarray(dg, np.int16); assert dg.shape == ang.shape
+    dxc, dyc = _sizes(dx, dy, dxc, dyc, ny)
+    out = np.empty((ny, nx), np.float32)
+    with _Outlets(outlets):
+        assert lib().orc_dinfconclimaccum(_p(ang), _p(dm), _p(q), _p(dg), _p(out), nx, ny, nodata, dm_nodata, q_nodata, csol, int(contcheck),
+                                          _p(dxc), _p(dyc)) == 0
+    return out
+
+
+def dinftranslimaccum(ang, tsup, tc, cs=None, dx=30.0, dy=30.0, nodata=MISSINGFLOAT, tsup_nodata=-9999.0, tc_nodata=-9999.0, cs_nodata=-9999.0,
+                      contcheck=True, outlets=None, dxc=None, dyc=None):
+    """(tla, tdep, ctpt); ctpt is None without cs"""
+    ang = np.ascontiguousarray(ang, np.float32); ny, nx = ang.shape
+    tsup, tc = _f32(tsup, ang.shape), _f32(tc, ang.shape)
+    c = None if cs is None else _f32(cs, ang.shape)
+    dxc, dyc = _sizes(dx, dy, dxc, dyc, ny)
+    tla, dep = np.empty((ny, nx), np.float32), np.empty((ny, nx), np.float32)
+    cout = None if c is None else np.empty((ny, nx), np.float32)
+    with _Outlets(outlets):
+        assert lib().orc_dinftranslimaccum(_p(ang), _p(tsup), _p(tc), _p(c), _p(tla), _p(dep), _p(cout), nx, ny, nodata, tsup_nodata, tc_nodata, cs_nodata,
+                                           int(contcheck), _p(dxc), _p(dyc)) == 0
+    return tla, dep, cout

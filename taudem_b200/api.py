@@ -198,14 +198,15 @@ def dinfdecayaccum_grid(ang, dm, weights=None, dx=30.0, dy=30.0, nodata=float(MI
 
 
 def dinfconclimaccum_grid(ang, dm, q, dg, csol=1.0, dx=30.0, dy=30.0, nodata=float(MISSINGFLOAT), dm_nodata=-9999.0, q_nodata=-9999.0, contcheck=True,
-                          outlets=None):
+                          outlets=None, dxc=None, dyc=None):
     """Concentration limited accumulation on the D-infinity flow field (td_dinfconclimaccum_host; src/DinfConcLimAccum.cpp:242-270):
     cells with q > 0 only; an indicator cell (dg > 0) has the concentration csol, any other the float sum of p * ctpt * q * dm over its
     contributors divided by its own q.  nodata = -FLT_MAX."""
     ang = _grid(ang, np.float32); dm = _grid(dm, np.float32); q = _grid(q, np.float32); dg = _grid(dg, np.int16)
     ny, nx = ang.shape
     assert dm.shape == ang.shape and q.shape == ang.shape and dg.shape == ang.shape
-    dxc, dyc = _rows(dx, ny), _rows(dy, ny)
+    dxc = _rows(dx, ny) if dxc is None else _rows(dxc, ny)
+    dyc = _rows(dy, ny) if dyc is None else _rows(dyc, ny)
     out = np.empty((ny, nx), np.float32)
     oc, orow, nout = _outlet_args(outlets)
     check(lib().td_dinfconclimaccum_host(_ptr(ang), _ptr(dm), _ptr(q), _ptr(dg), _ptr(out), nx, ny, np.float32(nodata), np.float32(dm_nodata), np.float32(q_nodata),
@@ -214,14 +215,15 @@ def dinfconclimaccum_grid(ang, dm, q, dg, csol=1.0, dx=30.0, dy=30.0, nodata=flo
 
 
 def dinftranslimaccum_grid(ang, tsup, tc, cs=None, dx=30.0, dy=30.0, nodata=float(MISSINGFLOAT), tsup_nodata=-9999.0, tc_nodata=-9999.0, cs_nodata=-9999.0,
-                           contcheck=True, outlets=None):
+                           contcheck=True, outlets=None, dxc=None, dyc=None):
     """Transport limited accumulation on the D-infinity flow field (td_dinftranslimaccum_host; src/DinfTransLimAccum.cpp:237-302):
     returns (tla, tdep, ctpt) — ctpt is None without a supply concentration grid `cs`.  nodata = -FLT_MAX."""
     ang = _grid(ang, np.float32); tsup = _grid(tsup, np.float32); tc = _grid(tc, np.float32)
     ny, nx = ang.shape
     assert tsup.shape == ang.shape and tc.shape == ang.shape
     c = None if cs is None else _grid(cs, np.float32)
-    dxc, dyc = _rows(dx, ny), _rows(dy, ny)
+    dxc = _rows(dx, ny) if dxc is None else _rows(dxc, ny)
+    dyc = _rows(dy, ny) if dyc is None else _rows(dyc, ny)
     tla = np.empty((ny, nx), np.float32); dep = np.empty((ny, nx), np.float32)
     cout = None if cs is None else np.empty((ny, nx), np.float32)
     oc, orow, nout = _outlet_args(outlets)

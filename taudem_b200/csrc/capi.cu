@@ -688,7 +688,7 @@ int td_gridnet_host(const int16_t* p, const int32_t* mask, int thresh, float* pl
     else {
       TD_CUDA(ctx->io[2].ensure(n * 2));
       int16_t* d_g = ctx->io[2].as<int16_t>();
-      if (int rc = td::launch_gord_finish(d_a, d_p, d_g, ss, p_nodata, nout >= 0 ? 1 : 0, st)) return rc;
+      if (int rc = td::launch_gord_finish(d_a, d_p, d_ok, ctx->node.as<unsigned short>(), d_g, ss, p_nodata, nout >= 0 ? 1 : 0, st)) return rc;
       TD_CUDA(d2h(gord, d_g, s, st));
     }
   }

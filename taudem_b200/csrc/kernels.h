@@ -46,7 +46,8 @@ int launch_slopearea(const float* slp, const float* sca, float* sa, const Strip&
 int launch_slopearearatio(const float* slp, const float* sca, float* sar, const Strip& s, float sca_nodata, cudaStream_t st);
 int launch_twi(const float* slp, const float* sca, float* twi, const Strip& s, float slp_nodata, float sca_nodata, cudaStream_t st);
 int launch_mask_ok(const int* mask, float* ok, const Strip& s, int thresh, cudaStream_t st);
-int launch_gord_finish(const float* g, const short* p, short* gord, const Strip& s, short p_nodata, int outlets, cudaStream_t st);
+int launch_gord_finish(const float* g, const short* p, const float* ok, const unsigned short* node, short* gord, const Strip& s, short p_nodata,
+                       int outlets, cudaStream_t st);
 cudaError_t launch_gen_dem(float* dem, const Strip& s, int row0, int total_ny, unsigned seed, float hurst, float tilt, cudaStream_t st);
 cudaError_t launch_gen_w(float* w, const Strip& s, int row0, unsigned seed, cudaStream_t st);
 }  // namespace td

@@ -1,9 +1,12 @@
 """The reference tools' outputs that the tests compare against, without the reference tools (oracle/_ref is built only
 where the reference sources are).  tests/golden/reference.json stores a digest of each output, keyed by a digest of the
-call.  `RefPipeline` has refrun.RefPipeline's interface and writes the same input files; it replays: pitremove, d8flowdir,
-dinfflowdir, aread8 and areadinf are recomputed by the C restatement (oracle/port), twi and slopearea with libm's logf /
-powf, and must match the stored digest bit for bit; the other tools return a Digest for util.assert_bits.
-TD_RECORD_REFERENCE=<file> with oracle/_ref built runs the tools instead and writes the digests to <file> at exit.
+call.  `RefPipeline` has refrun.RefPipeline's interface and writes the same input files; it replays: every tool is recomputed
+— pitremove, d8flowdir, dinfflowdir, aread8, areadinf and the five sibling sweep tools (d8flowpathextremeup, gridnet,
+dinfdecayaccum, dinfconclimaccum, dinftranslimaccum) by the C restatement (oracle/port), twi, slopearea, threshold and
+slopearearatio in numpy with libm's logf / powf — and must match the stored digest bit for bit.  `replayed` collects the keys
+of the calls whose outputs were recomputed and matched.
+TD_RECORD_REFERENCE=<file> with oracle/_ref built runs the tools instead, requires the recomputed outputs to be theirs too, and
+writes the digests to <file> at exit.
 """
 import atexit
 import ctypes
@@ -22,6 +25,7 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref
 RECORD = os.environ.get("TD_RECORD_REFERENCE")
 _recorded = {}
 _stored = None
+replayed = {}          # call key -> tool, for every call whose recomputed outputs matched the stored digests
 
 
 class Digest:
@@ -115,6 +119,20 @@ def _slopearea(slp, sca, m=None, n=None):
     return out
 
 
+def _threshold(ssa, thresh, mask=None, nodata=-1.0):
+    """Threshold: 1 where ssa >= thresh (and mask >= 0), else 0; MISSINGSHORT where ssa is nodata"""
+    ssa = np.asarray(ssa, np.float32)
+    ok = (ssa >= np.float32(thresh)) & (True if mask is None else np.asarray(mask, np.float32) >= 0)
+    return np.where(np.abs(ssa - np.float32(nodata)) < np.float32(1e-5), np.int16(-32768), ok.astype(np.int16)).astype(np.int16)
+
+
+def _slopearearatio(slp, sca, nodata=-1.0):
+    """SlopeAreaRatio: slp / sca in float where sca is data, else nodata (-1)"""
+    slp, sca = np.asarray(slp, np.float32), np.asarray(sca, np.float32)
+    with np.errstate(all="ignore"):
+        return np.where(np.abs(sca - np.float32(nodata)) < np.float32(1e-5), np.float32(-1.0), slp / sca).astype(np.float32)
+
+
 class RefPipeline:
     """refrun.RefPipeline's calls: the reference tools when recording, their stored outputs otherwise (module docstring)."""
 
@@ -153,11 +171,29 @@ class RefPipeline:
         if tool == "areadinf":
             kw.pop("w_nodata", None)
             return port.areadinf(*args, dx=dx, dy=dy, **kw)
+        if tool == "d8flowpathextremeup":
+            kw.pop("sa_nodata", None)                       # the sa values are taken as they are, nodata or not
+            return port.d8flowpathextremeup(*args, **kw)
+        if tool == "gridnet":
+            return port.gridnet(*args, dx=dx, dy=dy, **kw)
+        if tool == "dinfdecayaccum":
+            kw.pop("w_nodata", None)                        # (likewise the weights)
+            return port.dinfdecayaccum(*args, dx=dx, dy=dy, **kw)
+        if tool == "dinfconclimaccum":                      # nodata: of dm and q (the angles' is MISSINGFLOAT)
+            nd = kw.pop("nodata", -9999.0)
+            return port.dinfconclimaccum(*args, dx=dx, dy=dy, dm_nodata=nd, q_nodata=nd, **kw)
+        if tool == "dinftranslimaccum":                     # nodata: of tsup, tc and cs
+            nd = kw.pop("nodata", -9999.0)
+            return port.dinftranslimaccum(*args, dx=dx, dy=dy, tsup_nodata=nd, tc_nodata=nd, cs_nodata=nd, **kw)
         if tool == "twi":
             return _twi(*args, **kw)
         if tool == "slopearea":
             return _slopearea(*args, **kw)
-        return None
+        if tool == "threshold":
+            return _threshold(*args, **kw)
+        if tool == "slopearearatio":
+            return _slopearearatio(*args, **kw)
+        raise AssertionError(f"{tool}: no restatement")
 
     def _call(self, tool, args, kw):
         key = call_key(tool, self.dx, self.dy, self.np_ranks, args, kw)
@@ -166,7 +202,7 @@ class RefPipeline:
         if RECORD:
             _recorded[key] = [None if o is None else digest(o) for o in (out if many else (out,))]
             mine = self._restate(tool, args, kw)
-            if mine is not None and [digest(m) for m in (mine if many else (mine,))] != _recorded[key]:
+            if [None if m is None else digest(m) for m in (mine if many else (mine,))] != _recorded[key]:
                 raise AssertionError(f"{tool}: the restatement does not reproduce the reference's output")
             return out
         want = stored().get(key)
@@ -174,12 +210,11 @@ class RefPipeline:
             raise AssertionError(f"{tool}: no stored reference output for these inputs in {GOLDEN} "
                                  "(record it with TD_RECORD_REFERENCE=<file> where oracle/_ref is built)")
         mine = self._restate(tool, args, kw)
-        if mine is None:
-            res = tuple(None if h is None else Digest(h, f"{tool}[{i}]") for i, h in enumerate(want))
-        else:
-            res = mine if isinstance(mine, tuple) else (mine,)
-            for i, (r, h) in enumerate(zip(res, want)):
-                assert digest(r) == h, f"{tool}[{i}]: the restatement no longer reproduces the reference's output"
+        res = mine if isinstance(mine, tuple) else (mine,)
+        assert len(res) == len(want), f"{tool}: {len(res)} outputs, {len(want)} stored"
+        for i, (r, h) in enumerate(zip(res, want)):
+            assert (None if r is None else digest(r)) == h, f"{tool}[{i}]: the restatement no longer reproduces the reference's output"
+        replayed[key] = tool
         return res if many else res[0]
 
 

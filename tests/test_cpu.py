@@ -231,6 +231,129 @@ def test_c_restatement_reproduces_golden(name):
     assert_bits(port.areadinf(g["ang"], dx=dx, dy=dy, contcheck=False), g["sca_nc"], "sca_nc")
 
 
+def test_c_restatement_reproduces_the_sibling_golden():
+    """Pins the restatement of the sibling sweep tools and the point-wise consumers: every array of tests/golden/siblings.npz (outputs
+    of the reference executables on the hills_holes rasters, 30 x 20 m cells) recomputed bit for bit."""
+    import port
+    import reference
+    if not port.available():
+        pytest.skip("oracle/port not built")
+    g, x = load_golden("hills_holes"), load_golden("siblings")
+    p, ang, dx, dy = g["p"], g["ang"], float(g["dx"]), float(g["dy"])
+    got = {"ssa_max": port.d8flowpathextremeup(p, x["sa"]), "ssa_min_nc": port.d8flowpathextremeup(p, x["sa"], usemax=False, contcheck=False),
+           "dsca": port.dinfdecayaccum(ang, x["dm"], dx=dx, dy=dy),
+           "dsca_w_nc": port.dinfdecayaccum(ang, x["dm"], weights=g["w"], contcheck=False, dx=dx, dy=dy),
+           "ctpt": port.dinfconclimaccum(ang, x["dm"], x["q"], x["dg"], csol=2.5, dx=dx, dy=dy),
+           "ctpt_nc": port.dinfconclimaccum(ang, x["dm"], x["q"], x["dg"], csol=2.5, contcheck=False, dx=dx, dy=dy),
+           "src": reference._threshold(g["ad8"], 50.0), "twi": reference._twi(g["slp"], g["sca"]),
+           "sa_default": reference._slopearea(g["slp"], g["sca"]), "sar": reference._slopearearatio(g["slp"], g["sca"])}
+    got["plen"], got["tlen"], got["gord"] = port.gridnet(p, dx=dx, dy=dy)
+    got["plen_m"], got["tlen_m"], got["gord_m"] = port.gridnet(p, mask=x["gn_mask"], thresh=5, dx=dx, dy=dy)
+    got["tla"], got["tdep"], none = port.dinftranslimaccum(ang, x["q"], x["tc"], dx=dx, dy=dy)
+    got["tla_c"], got["tdep_c"], got["ctpt_c"] = port.dinftranslimaccum(ang, x["q"], x["tc"], cs=x["cs"], contcheck=False, dx=dx, dy=dy)
+    assert none is None
+    inputs = {"q", "dm", "dg", "tc", "cs", "sa", "gn_mask"}
+    assert set(got) == set(x) - inputs
+    for k in sorted(got):
+        assert_bits(got[k], x[k], k)
+    assert (x["gord"] >= 3).any() and (x["ctpt"] == 2.5).any() and (x["tdep"] > 0).any()      # the vectors are not trivial
+
+
+def test_c_restatement_reproduces_every_stored_sibling_output(refrun, tmp_path):
+    """Every reference output the GPU sibling tests compare against (tests/sibling_cases.py; tests/golden/reference.json), recomputed by
+    the restatement on the CPU and matched to its stored digest.  The count is asserted: a call that is not replayed fails here."""
+    import port
+    import reference
+    if not port.available():
+        pytest.skip("oracle/port not built")
+    import sibling_cases
+    keys = set()
+    for i, case in enumerate(sibling_cases.CASES):
+        d = tmp_path / str(i)
+        d.mkdir()
+        _, calls = case(d)
+        R = refrun.RefPipeline(workdir=str(d))
+        for label, tool, args, kw in calls:
+            before = set(reference.replayed)
+            out = getattr(R, tool)(*args, **kw)
+            new = set(reference.replayed) - before
+            assert len(new) <= 1 and all(reference.replayed[k] == tool for k in new), (label, tool)
+            assert all(o is None or isinstance(o, np.ndarray) for o in (out if isinstance(out, tuple) else (out,))), (label, tool)
+            keys.add(reference.call_key(tool, R.dx, R.dy, R.np_ranks, args, kw))
+    assert all(reference.replayed.get(k) for k in keys)
+    assert len(keys) == sum(len(case(tmp_path)[1]) for case in sibling_cases.CASES) == 18
+
+
+def _random_sibling_grids(rng, ny, nx):
+    """A D8 grid (codes 0..8, flats unresolved, nodata border and holes) and a D-infinity angle grid (flats, nodata, arbitrary angles)
+    of a random DEM, and value grids with nodata, zero and negative values"""
+    import port
+    dem = (rng.random((ny, nx)) * 20).astype(np.float32)
+    dem[rng.random((ny, nx)) < 0.15] = 5.0                       # flats
+    dem[rng.random((ny, nx)) < 0.03] = -9999.0
+    fel = port.pitremove(dem)
+    p, _ = port.d8flowdir(fel, dx=10.0, dy=13.0, flats=False)
+    p[0, :] = p[-1, :] = p[:, 0] = p[:, -1] = -32768             # (gridnet reads past its arrays at the grid edge)
+    ang, _ = port.dinfflowdir(fel, dx=10.0, dy=13.0, flats=False)
+    odd = rng.random((ny, nx)) < 0.03
+    ang[odd] = (rng.random(odd.sum()) * 6.4).astype(np.float32)
+    def vals(lo, hi, nd=0.03):
+        v = rng.uniform(lo, hi, (ny, nx)).astype(np.float32)
+        v[rng.random((ny, nx)) < 0.05] = 0.0
+        v[rng.random((ny, nx)) < nd] = -9999.0
+        return v
+    return p, ang, vals
+
+
+def test_c_restatement_matches_the_live_reference_sibling_tools(tmp_path, monkeypatch):
+    """Where oracle/_ref is built: the restatement of the five sibling sweep tools against the reference executables, live, on small
+    random grids with nodata, unresolved flats, arbitrary angles, zero and negative values, per-row options and outlets."""
+    import port
+    import refrun
+    if not (refrun.available() and port.available() and os.access(os.path.join(refrun.REF, "gridnet"), os.X_OK)):
+        pytest.skip("oracle/_ref not built")
+    from util import write_point_shapefile
+    rng = np.random.default_rng(123)
+    monkeypatch.setattr(refrun, "INPUTS_ONLY", False)
+    for ny, nx in ((23, 31), (40, 57), (64, 35)):
+        p, ang, vals = _random_sibling_grids(rng, ny, nx)
+        R = refrun.RefPipeline(workdir=str(tmp_path), dx=10.0, dy=13.0)
+        sa = vals(-50.0, 50.0)
+        oc, orr = [int(c) for c in rng.integers(0, nx, 3)], [int(r) for r in rng.integers(0, ny, 3)]
+        shp = str(tmp_path / "o.shp")
+        write_point_shapefile(shp, [(c + 0.5) * 10.0 for c in oc], [13.0 * ny - (r + 0.5) * 13.0 for r in orr])
+        outs = (oc, orr)
+        for usemax in (True, False):
+            for cont in (True, False):
+                assert_bits(port.d8flowpathextremeup(p, sa, usemax=usemax, contcheck=cont), R.d8flowpathextremeup(p, sa, usemax=usemax, contcheck=cont),
+                            f"ssa {usemax} {cont} {ny}x{nx}")
+        assert_bits(port.d8flowpathextremeup(p, sa, outlets=outs), R.d8flowpathextremeup(p, sa, outlets=shp), f"ssa -o {ny}x{nx}")
+        mask = rng.integers(-2, 6, (ny, nx)).astype(np.int32)
+        for kw in ({}, {"mask": mask, "thresh": 2}):
+            for o, r, n in zip(port.gridnet(p, dx=10.0, dy=13.0, **kw), R.gridnet(p, **kw), ("plen", "tlen", "gord")):
+                assert_bits(o, r, f"{n} {sorted(kw)} {ny}x{nx}")
+            for o, r, n in zip(port.gridnet(p, dx=10.0, dy=13.0, outlets=outs, **kw), R.gridnet(p, outlets=shp, **kw), ("plen", "tlen", "gord")):
+                assert_bits(o, r, f"{n} -o {sorted(kw)} {ny}x{nx}")
+        dm, w, q, tc, cs = vals(-0.5, 1.5), vals(-1.0, 2.0), vals(-1.0, 3.0), vals(-1.0, 6.0), vals(-0.5, 2.0)
+        dg = (rng.random((ny, nx)) < 0.1).astype(np.int16)
+        for cont in (True, False):
+            assert_bits(port.dinfdecayaccum(ang, dm, dx=10.0, dy=13.0, contcheck=cont), R.dinfdecayaccum(ang, dm, contcheck=cont), f"dsca {cont}")
+            assert_bits(port.dinfdecayaccum(ang, dm, weights=w, dx=10.0, dy=13.0, contcheck=cont), R.dinfdecayaccum(ang, dm, weights=w, contcheck=cont),
+                        f"dsca -wg {cont}")
+            assert_bits(port.dinfconclimaccum(ang, dm, q, dg, csol=1.5, dx=10.0, dy=13.0, contcheck=cont),
+                        R.dinfconclimaccum(ang, dm, q, dg, csol=1.5, contcheck=cont), f"ctpt {cont}")
+            for c in (None, cs):
+                for o, r, n in zip(port.dinftranslimaccum(ang, q, tc, cs=c, dx=10.0, dy=13.0, contcheck=cont), R.dinftranslimaccum(ang, q, tc, cs=c, contcheck=cont),
+                                   ("tla", "tdep", "ctpt")):
+                    if r is not None:
+                        assert_bits(o, r, f"{n} cs={c is not None} {cont}")
+        assert_bits(port.dinfdecayaccum(ang, dm, dx=10.0, dy=13.0, outlets=outs), R.dinfdecayaccum(ang, dm, outlets=shp), "dsca -o")
+        assert_bits(port.dinfconclimaccum(ang, dm, q, dg, dx=10.0, dy=13.0, outlets=outs), R.dinfconclimaccum(ang, dm, q, dg, outlets=shp), "ctpt -o")
+        for o, r, n in zip(port.dinftranslimaccum(ang, q, tc, cs=cs, dx=10.0, dy=13.0, outlets=outs), R.dinftranslimaccum(ang, q, tc, cs=cs, outlets=shp),
+                           ("tla", "tdep", "ctpt")):
+            assert_bits(o, r, n + " -o")
+
+
 def test_geographic_cell_sizes_match_reference(refrun, tmp_path):
     """Geographic rasters: our per-row dxc/dyc (tiff_io cell_sizes) fed to the C restatement reproduce the recorded outputs of
     the reference tools on the same file (they derive the sizes themselves in tiffIO)."""

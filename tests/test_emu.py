@@ -569,11 +569,13 @@ def test_emulated_sweeps_on_a_larger_grid(emu):
 
 def test_emulated_random_configurations(emu):
     """A short deterministic slice of scripts/emu_stress.py: random grid sizes, flats, holes, strip counts, sweeps and strip
-    flats against the oracle."""
+    flats against the oracle; every sibling algebra 1-9 at least once on random value grids."""
     import sys
     r = subprocess.run([sys.executable, os.path.join(ROOT, "scripts", "emu_stress.py"), "777", "14", "120"], stdout=subprocess.PIPE,
                        stderr=subprocess.STDOUT, text=True, timeout=600)
     assert r.returncode == 0 and " bad 0 " in r.stdout, r.stdout[-2000:]
+    runs = r.stdout.split("algebra runs ")[1].split()[0]
+    assert all(int(n) >= 1 for n in runs.split(",")) and len(runs.split(",")) == 9, r.stdout[-2000:]
 
 
 def test_emulated_sibling_tools_on_the_golden_vectors(emu):

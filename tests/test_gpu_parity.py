@@ -7,11 +7,13 @@ import numpy as np
 import pytest
 
 import port
+import sibling_cases
 import taudem_b200 as td
 from taudem_b200 import synth
 from util import ANG_ND, FEL_ND, assert_bits, assert_float_parity, golden_cases, load_golden, write_geographic_dem
 
 pytestmark = pytest.mark.gpu
+MISSINGFLOAT = np.float32(-3.4028234663852886e38)
 
 
 @pytest.mark.parametrize("name", golden_cases())
@@ -201,14 +203,21 @@ def test_properties_large():
     assert ad8[valid].min() >= 1.0
 
 
-def test_sweep_with_many_tile_crossings_matches_the_reference(refrun):
+@pytest.fixture(scope="module")
+def crossings():
+    """the 2100 x 3000 DEM of the tile-crossing tests: (fel, p, sd8, ang) of the C restatement"""
+    dem = synth.punch_holes(synth.gen_dem(2100, 3000, hurst=0.8, tilt=1.0, seed=9))
+    fel = port.pitremove(dem)
+    p, sd8 = port.d8flowdir(fel)
+    ang, _ = port.dinfflowdir(fel)
+    return fel, p, sd8, ang
+
+
+def test_sweep_with_many_tile_crossings_matches_the_reference(refrun, crossings):
     """2100 x 3000 cells (6 200 tiles of the dataflow sweep, rivers that cross hundreds of tiles, thousands of tile
     re-activations): ad8 bit for bit, sca within the tolerance, with and without weights, against the reference tools."""
-    dem = synth.punch_holes(synth.gen_dem(2100, 3000, hurst=0.8, tilt=1.0, seed=9))
-    w = synth.gen_weights(*dem.shape)
-    fel = port.pitremove(dem)
-    p, _ = port.d8flowdir(fel)
-    ang, _ = port.dinfflowdir(fel)
+    fel, p, _, ang = crossings
+    w = synth.gen_weights(*p.shape)
     R = refrun.RefPipeline(np_ranks=8)
     ad8 = td.aread8_grid(p)
     assert_bits(ad8, R.aread8(p), "ad8")
@@ -392,168 +401,103 @@ def test_overlapped_two_tool_call_equals_the_two_calls():
     assert_bits(sca, td.areadinf_grid(ang, dx=25.0, dy=35.0, contcheck=False), "sca -nc (overlapped call)")
 
 
-def test_d8_flow_path_extreme_up(refrun, tmp_path):
-    """d8flowpathextremeup (SURVEY.md 8(f) rank 3: a sibling of aread8 on the same sweep) against the reference executable
-    (oracle/_ref/d8flowpathextremeup): max, min, -nc, outlets; grid level and our executable, bit for bit."""
+def _bin(tool):
     import os
+    return os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "taudem_b200", "bin", tool)
+
+
+def _run(tool, *args):
     import subprocess
-    from util import write_point_shapefile
-    dem = synth.punch_holes(synth.gen_dem(330, 410, hurst=0.8, tilt=1.0, seed=41))
-    fel = port.pitremove(dem); p, sd8 = port.d8flowdir(fel)
-    sa = np.where(sd8 < 0, np.float32(0.0), sd8).astype(np.float32)           # "largest slope upstream"
-    R = refrun.RefPipeline(workdir=str(tmp_path))
-    assert_bits(td.d8flowpathextremeup_grid(p, sa), R.d8flowpathextremeup(p, sa), "ssa max")
-    assert_bits(td.d8flowpathextremeup_grid(p, fel, usemax=False, contcheck=False), R.d8flowpathextremeup(p, fel, usemax=False, contcheck=False), "ssa min -nc")
-    ny, nx = p.shape
-    order = np.argsort(port.aread8(p, contcheck=False).ravel())
-    cells = [int(order[-1]), int(order[-40]), int(order[-700])]
-    cols = [c % nx for c in cells]; rows = [c // nx for c in cells]
-    dx = dy = 30.0
-    shp = str(tmp_path / "outlets.shp")
-    write_point_shapefile(shp, [(c + 0.5) * dx for c in cols], [dy * ny - (r + 0.5) * dy for r in rows])
-    ref = R.d8flowpathextremeup(p, sa, outlets=shp)
-    assert_bits(td.d8flowpathextremeup_grid(p, sa, outlets=(cols, rows)), ref, "ssa max -o")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    r = subprocess.run([_bin(tool)] + [str(a) for a in args], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    assert r.returncode == 0 and "rror" not in r.stdout, r.stdout
+
+
+def _reference(refrun, calls, workdir):
+    """the reference outputs of a sibling case's calls (tests/sibling_cases.py), by label"""
+    R = refrun.RefPipeline(workdir=str(workdir))
+    return {label: getattr(R, tool)(*args, **kw) for label, tool, args, kw in calls}
+
+
+def test_d8_flow_path_extreme_up(refrun, tmp_path):
+    """d8flowpathextremeup (SURVEY.md 8(f) rank 3: a sibling of aread8 on the same sweep) against the reference's outputs (replayed by
+    the C restatement, tests/reference.py): max, min, -nc, outlets; grid level and our executable, bit for bit."""
+    x, calls = sibling_cases.flowpathextremeup(tmp_path)
+    ref = _reference(refrun, calls, tmp_path)
+    p, sa, outs = x["p"], x["sa"], (x["cols"], x["rows"])
+    assert_bits(td.d8flowpathextremeup_grid(p, sa), ref["ssa max"], "ssa max")
+    assert_bits(td.d8flowpathextremeup_grid(p, x["fel"], usemax=False, contcheck=False), ref["ssa min -nc"], "ssa min -nc")
+    assert_bits(td.d8flowpathextremeup_grid(p, sa, outlets=outs), ref["ssa max -o"], "ssa max -o")
     out = str(tmp_path / "ours_ssa.tif")
-    r = subprocess.run([os.path.join(root, "taudem_b200", "bin", "d8flowpathextremeup"), "-p", str(tmp_path / "pin.tif"), "-sa", str(tmp_path / "sa.tif"),
-                        "-ssa", out, "-o", shp], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert r.returncode == 0, r.stdout
-    assert_bits(td.read_raster(out), ref, "d8flowpathextremeup -o (files)")
+    _run("d8flowpathextremeup", "-p", tmp_path / "pin.tif", "-sa", tmp_path / "sa.tif", "-ssa", out, "-o", x["shp"])
+    assert_bits(td.read_raster(out), ref["ssa max -o"], "d8flowpathextremeup -o (files)")
 
 
 def test_gridnet(refrun, tmp_path):
-    """gridnet (SURVEY.md 8(f) rank 3: a sibling of aread8 on the same sweep) against the reference executable (oracle/_ref/gridnet):
-    plain, mask + threshold, outlets, outlets + mask; grid level and our executable, bit for bit."""
-    import os
-    import subprocess
-    from util import write_point_shapefile
-    dem = synth.punch_holes(synth.gen_dem(330, 410, hurst=0.8, tilt=1.0, seed=47))
-    fel = port.pitremove(dem); p, _ = port.d8flowdir(fel)
-    R = refrun.RefPipeline(workdir=str(tmp_path))
+    """gridnet (SURVEY.md 8(f) rank 3: a sibling of aread8 on the same sweep) against the reference's outputs: plain, mask + threshold,
+    outlets, outlets + mask; grid level and our executable, bit for bit."""
+    x, calls = sibling_cases.gridnet(tmp_path)
+    ref = _reference(refrun, calls, tmp_path)
+    p, mask, outs = x["p"], x["mask"], (x["cols"], x["rows"])
 
-    def same(ours, ref, what):
-        for a, b, n in zip(ours, ref, ("plen", "tlen", "gord")):
+    def same(ours, want, what):
+        for a, b, n in zip(ours, want, ("plen", "tlen", "gord")):
             assert_bits(a, b, f"{n} {what}")
 
-    same(td.gridnet_grid(p), R.gridnet(p), "")
-    ad8 = port.aread8(p, contcheck=False)
-    mask = np.where(ad8 >= 0, ad8, 0).astype(np.int32)
-    same(td.gridnet_grid(p, mask=mask, thresh=20), R.gridnet(p, mask=mask, thresh=20), "-mask -thresh 20")
-    ny, nx = p.shape
-    order = np.argsort(ad8.ravel())
-    cells = [int(order[-1]), int(order[-40]), int(order[-700])]
-    cols = [c % nx for c in cells]; rows = [c // nx for c in cells]
-    dx = dy = 30.0
-    shp = str(tmp_path / "outlets.shp")
-    write_point_shapefile(shp, [(c + 0.5) * dx for c in cols], [dy * ny - (r + 0.5) * dy for r in rows])
-    same(td.gridnet_grid(p, outlets=(cols, rows)), R.gridnet(p, outlets=shp), "-o")
-    ref = R.gridnet(p, mask=mask, thresh=20, outlets=shp)
-    same(td.gridnet_grid(p, mask=mask, thresh=20, outlets=(cols, rows)), ref, "-o -mask")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    same(td.gridnet_grid(p), ref[""], "")
+    same(td.gridnet_grid(p, mask=mask, thresh=20), ref["-mask -thresh 20"], "-mask -thresh 20")
+    same(td.gridnet_grid(p, outlets=outs), ref["-o"], "-o")
+    same(td.gridnet_grid(p, mask=mask, thresh=20, outlets=outs), ref["-o -mask"], "-o -mask")
     o = {n: str(tmp_path / f"ours_{n}.tif") for n in ("plen", "tlen", "gord")}
-    r = subprocess.run([os.path.join(root, "taudem_b200", "bin", "gridnet"), "-p", str(tmp_path / "pin.tif"), "-plen", o["plen"], "-tlen", o["tlen"], "-gord", o["gord"],
-                        "-o", shp, "-mask", str(tmp_path / "mask.tif"), "-thresh", "20"], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert r.returncode == 0 and "error" not in r.stdout.lower(), r.stdout
-    same((td.read_raster(o["plen"]), td.read_raster(o["tlen"]), td.read_raster(o["gord"], np.int16)), ref, "-o -mask (files)")
+    _run("gridnet", "-p", tmp_path / "pin.tif", "-plen", o["plen"], "-tlen", o["tlen"], "-gord", o["gord"], "-o", x["shp"], "-mask", tmp_path / "mask.tif",
+         "-thresh", "20")
+    same((td.read_raster(o["plen"]), td.read_raster(o["tlen"]), td.read_raster(o["gord"], np.int16)), ref["-o -mask"], "-o -mask (files)")
 
 
 def test_dinf_decay_accumulation(refrun, tmp_path):
-    """dinfdecayaccum (SURVEY.md 8(f) rank 3: a sibling of areadinf on the same sweep) against the reference executable
-    (oracle/_ref/dinfdecayaccum): plain, weights + -nc, nodata multipliers, outlets; grid level and our executable, bit for bit."""
-    import os
-    import subprocess
-    from util import write_point_shapefile
-    dem = synth.punch_holes(synth.gen_dem(330, 410, hurst=0.8, tilt=1.0, seed=43))
-    fel = port.pitremove(dem); ang, slp = port.dinfflowdir(fel)
-    rng = np.random.default_rng(9)
-    dm = rng.uniform(0.3, 1.0, ang.shape).astype(np.float32)
-    dm[rng.random(ang.shape) < 0.001] = -9999.0
-    w = rng.uniform(0.0, 2.0, ang.shape).astype(np.float32)
-    R = refrun.RefPipeline(workdir=str(tmp_path))
-    assert_bits(td.dinfdecayaccum_grid(ang, dm), R.dinfdecayaccum(ang, dm), "dsca")
-    assert_bits(td.dinfdecayaccum_grid(ang, dm, weights=w, contcheck=False), R.dinfdecayaccum(ang, dm, weights=w, contcheck=False), "dsca -wg -nc")
-    ny, nx = ang.shape
-    order = np.argsort(port.areadinf(ang, contcheck=False).ravel())
-    cells = [int(order[-1]), int(order[-40]), int(order[-700])]
-    cols = [c % nx for c in cells]; rows = [c // nx for c in cells]
-    dx = dy = 30.0
-    shp = str(tmp_path / "outlets.shp")
-    write_point_shapefile(shp, [(c + 0.5) * dx for c in cols], [dy * ny - (r + 0.5) * dy for r in rows])
-    ref = R.dinfdecayaccum(ang, dm, outlets=shp)
-    assert_bits(td.dinfdecayaccum_grid(ang, dm, outlets=(cols, rows)), ref, "dsca -o")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    """dinfdecayaccum (SURVEY.md 8(f) rank 3: a sibling of areadinf on the same sweep) against the reference's outputs: plain,
+    weights + -nc, nodata multipliers, outlets; grid level and our executable, bit for bit."""
+    x, calls = sibling_cases.dinfdecayaccum(tmp_path)
+    ref = _reference(refrun, calls, tmp_path)
+    ang, dm = x["ang"], x["dm"]
+    assert_bits(td.dinfdecayaccum_grid(ang, dm), ref["dsca"], "dsca")
+    assert_bits(td.dinfdecayaccum_grid(ang, dm, weights=x["w"], contcheck=False), ref["dsca -wg -nc"], "dsca -wg -nc")
+    assert_bits(td.dinfdecayaccum_grid(ang, dm, outlets=(x["cols"], x["rows"])), ref["dsca -o"], "dsca -o")
     out = str(tmp_path / "ours_dsca.tif")
-    r = subprocess.run([os.path.join(root, "taudem_b200", "bin", "dinfdecayaccum"), "-ang", str(tmp_path / "angin.tif"), "-dm", str(tmp_path / "dm.tif"),
-                        "-dsca", out, "-o", shp], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert r.returncode == 0, r.stdout
-    assert_bits(td.read_raster(out), ref, "dinfdecayaccum -o (files)")
-
-
-def _sibling_inputs(shape, seed):
-    rng = np.random.default_rng(seed)
-    q = rng.uniform(0.5, 3.0, shape).astype(np.float32)
-    q[rng.random(shape) < 0.001] = -9999.0
-    q[rng.random(shape) < 0.001] = 0.0
-    dm = rng.uniform(0.2, 1.0, shape).astype(np.float32)
-    dm[rng.random(shape) < 0.0005] = -9999.0
-    dg = (rng.random(shape) < 0.02).astype(np.int16)
-    tc = rng.uniform(0.0, 8.0, shape).astype(np.float32)
-    tc[rng.random(shape) < 0.0005] = -9999.0
-    cs = rng.uniform(0.0, 2.0, shape).astype(np.float32)
-    cs[rng.random(shape) < 0.0005] = -9999.0
-    return q, dm, dg, tc, cs
+    _run("dinfdecayaccum", "-ang", tmp_path / "angin.tif", "-dm", tmp_path / "dm.tif", "-dsca", out, "-o", x["shp"])
+    assert_bits(td.read_raster(out), ref["dsca -o"], "dinfdecayaccum -o (files)")
 
 
 def test_dinf_conc_lim_and_trans_lim_accumulation(refrun, tmp_path):
     """DinfConcLimAccum and DinfTransLimAccum (SURVEY.md 8(f) rank 3: the last two siblings of areadinf on the same sweep) against the
-    reference executables (oracle/_ref/dinfconclimaccum, dinftranslimaccum): with and without contamination checking, with and without
-    the concentration that travels with the transport, outlets; grid level and our executables, bit for bit."""
-    import os
-    import subprocess
-    from util import write_point_shapefile
-    dem = synth.punch_holes(synth.gen_dem(340, 430, hurst=0.8, tilt=1.0, seed=47))
-    fel = port.pitremove(dem); ang, _ = port.dinfflowdir(fel)
-    q, dm, dg, tc, cs = _sibling_inputs(ang.shape, 11)
-    R = refrun.RefPipeline(workdir=str(tmp_path))
-    ny, nx = ang.shape
-    order = np.argsort(port.areadinf(ang, contcheck=False).ravel())
-    cells = [int(order[-1]), int(order[-40]), int(order[-700])]
-    cols = [c % nx for c in cells]; rows = [c // nx for c in cells]
-    dx = dy = 30.0
-    shp = str(tmp_path / "outlets.shp")
-    write_point_shapefile(shp, [(c + 0.5) * dx for c in cols], [dy * ny - (r + 0.5) * dy for r in rows])
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    reference's outputs: with and without contamination checking, with and without the concentration that travels with the transport,
+    outlets; grid level and our executables, bit for bit."""
+    x, calls = sibling_cases.conc_and_trans_lim(tmp_path)
+    ref = _reference(refrun, calls, tmp_path)
+    ang, q, dm, dg, tc, cs, outs = x["ang"], x["q"], x["dm"], x["dg"], x["tc"], x["cs"], (x["cols"], x["rows"])
     # concentration limited
-    assert_bits(td.dinfconclimaccum_grid(ang, dm, q, dg, csol=2.5), R.dinfconclimaccum(ang, dm, q, dg, csol=2.5), "ctpt")
-    assert_bits(td.dinfconclimaccum_grid(ang, dm, q, dg, contcheck=False), R.dinfconclimaccum(ang, dm, q, dg, contcheck=False), "ctpt -nc")
-    ref = R.dinfconclimaccum(ang, dm, q, dg, csol=0.75, contcheck=False, outlets=shp)
-    assert_bits(td.dinfconclimaccum_grid(ang, dm, q, dg, csol=0.75, contcheck=False, outlets=(cols, rows)), ref, "ctpt -o")
+    assert_bits(td.dinfconclimaccum_grid(ang, dm, q, dg, csol=2.5), ref["ctpt"], "ctpt")
+    assert_bits(td.dinfconclimaccum_grid(ang, dm, q, dg, contcheck=False), ref["ctpt -nc"], "ctpt -nc")
+    assert_bits(td.dinfconclimaccum_grid(ang, dm, q, dg, csol=0.75, contcheck=False, outlets=outs), ref["ctpt -o"], "ctpt -o")
     out = str(tmp_path / "ours_ctpt.tif")
-    r = subprocess.run([os.path.join(root, "taudem_b200", "bin", "dinfconclimaccum"), "-ang", str(tmp_path / "angin.tif"), "-dm", str(tmp_path / "dm.tif"),
-                        "-q", str(tmp_path / "q.tif"), "-dg", str(tmp_path / "dg.tif"), "-ctpt", out, "-csol", "0.75", "-nc", "-o", shp],
-                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert r.returncode == 0 and "rror" not in r.stdout, r.stdout
-    assert_bits(td.read_raster(out), ref, "dinfconclimaccum -o (files)")
-    MISSINGFLOAT = np.float32(-3.4028234663852886e38)
+    _run("dinfconclimaccum", "-ang", tmp_path / "angin.tif", "-dm", tmp_path / "dm.tif", "-q", tmp_path / "q.tif", "-dg", tmp_path / "dg.tif", "-ctpt", out,
+         "-csol", "0.75", "-nc", "-o", x["shp"])
+    assert_bits(td.read_raster(out), ref["ctpt -o"], "dinfconclimaccum -o (files)")
     assert (td.read_raster(out) != MISSINGFLOAT).mean() > 0.02
     # transport limited
     tsup = q
     for kw in ({}, {"contcheck": False}, {"cs": cs}, {"cs": cs, "contcheck": False}):
         ours = td.dinftranslimaccum_grid(ang, tsup, tc, **kw)
-        refs = R.dinftranslimaccum(ang, tsup, tc, **kw)
-        for o, f, name in zip(ours, refs, ("tla", "tdep", "ctpt")):
+        for o, f, name in zip(ours, ref[f"translim {sorted(kw)}"], ("tla", "tdep", "ctpt")):
             if f is not None:
                 assert_bits(o, f, f"{name} {kw.keys()}")
     assert (ours[0] != MISSINGFLOAT).mean() > 0.5 and (ours[1] > 0).mean() > 0.1
-    refs = R.dinftranslimaccum(ang, tsup, tc, cs=cs, contcheck=False, outlets=shp)
-    ours = td.dinftranslimaccum_grid(ang, tsup, tc, cs=cs, contcheck=False, outlets=(cols, rows))
+    refs = ref["translim -cs -nc -o"]
+    ours = td.dinftranslimaccum_grid(ang, tsup, tc, cs=cs, contcheck=False, outlets=outs)
     for o, f, name in zip(ours, refs, ("tla", "tdep", "ctpt")):
         assert_bits(o, f, name + " -o")
     outs = [str(tmp_path / f"ours_{n}.tif") for n in ("tla", "tdep", "ctptout")]
-    r = subprocess.run([os.path.join(root, "taudem_b200", "bin", "dinftranslimaccum"), "-ang", str(tmp_path / "angin.tif"), "-tsup", str(tmp_path / "tsup.tif"),
-                        "-tc", str(tmp_path / "tc.tif"), "-cs", str(tmp_path / "cs.tif"), "-ctpt", outs[2], "-tla", outs[0], "-tdep", outs[1], "-nc", "-o", shp],
-                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert r.returncode == 0 and "rror" not in r.stdout, r.stdout
+    _run("dinftranslimaccum", "-ang", tmp_path / "angin.tif", "-tsup", tmp_path / "tsup.tif", "-tc", tmp_path / "tc.tif", "-cs", tmp_path / "cs.tif",
+         "-ctpt", outs[2], "-tla", outs[0], "-tdep", outs[1], "-nc", "-o", x["shp"])
     for o, f, name in zip(outs, refs, ("tla", "tdep", "ctpt")):
         assert_bits(td.read_raster(o), f, name + " -o (files)")
 
@@ -669,3 +613,209 @@ def test_outlets_grid_and_file_level(refrun, tmp_path):
                            stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         assert r.returncode == 0, r.stdout
         assert_bits(td.read_raster(out), ref, f"{tool} -o (files)")
+
+
+# ---- the sibling sweep tools (algebras 1-9 of k_sweep_warp, sweep_warp.cu) against the C restatement (oracle/port), which the CPU suite
+#      pins on the reference's outputs: cell-level diffs at the shapes, sizes and values where the kernels could go wrong.
+def _sibling_values(rng, shape):
+    """value grids with nodata (-9999), zero and negative values"""
+    def vals(lo, hi, zero=0.03, nd=0.02):
+        v = rng.uniform(lo, hi, shape).astype(np.float32)
+        v[rng.random(shape) < zero] = 0.0
+        v[rng.random(shape) < nd] = -9999.0
+        return v
+    return dict(sa=vals(-50.0, 50.0), dm=vals(-0.2, 1.2), w=vals(-0.5, 2.0), q=vals(-0.5, 3.0), tc=vals(-0.5, 6.0), cs=vals(-0.2, 2.0),
+                dg=(rng.random(shape) < 0.05).astype(np.int16), mask=rng.integers(-1, 4, shape).astype(np.int32))
+
+
+def _check_siblings(p, ang, v, what, dx=30.0, dy=30.0, dxc=None, dyc=None, contchecks=(True, False), outlets=None, algs=range(1, 10), thresh=1):
+    """the nine algebras on (p, ang) with the value grids v, GPU against the restatement, bit for bit"""
+    sz = dict(dx=dx, dy=dy, dxc=dxc, dyc=dyc)
+    for cont in contchecks:
+        tag = f"{what} contcheck={cont}"
+        for alg, usemax in ((1, True), (2, False)):
+            if alg in algs:
+                assert_bits(td.d8flowpathextremeup_grid(p, v["sa"], usemax=usemax, contcheck=cont, outlets=outlets),
+                            port.d8flowpathextremeup(p, v["sa"], usemax=usemax, contcheck=cont, outlets=outlets), f"ssa usemax={usemax} {tag}")
+        if 3 in algs:
+            assert_bits(td.dinfdecayaccum_grid(ang, v["dm"], contcheck=cont, outlets=outlets, **sz),
+                        port.dinfdecayaccum(ang, v["dm"], contcheck=cont, outlets=outlets, **sz), f"dsca {tag}")
+            assert_bits(td.dinfdecayaccum_grid(ang, v["dm"], weights=v["w"], contcheck=cont, outlets=outlets, **sz),
+                        port.dinfdecayaccum(ang, v["dm"], weights=v["w"], contcheck=cont, outlets=outlets, **sz), f"dsca -wg {tag}")
+        if 7 in algs:
+            assert_bits(td.dinfconclimaccum_grid(ang, v["dm"], v["q"], v["dg"], csol=1.5, contcheck=cont, outlets=outlets, **sz),
+                        port.dinfconclimaccum(ang, v["dm"], v["q"], v["dg"], csol=1.5, contcheck=cont, outlets=outlets, **sz), f"ctpt {tag}")
+        for alg, cs in ((8, None), (9, v["cs"])):
+            if alg in algs:
+                for o, r, n in zip(td.dinftranslimaccum_grid(ang, v["q"], v["tc"], cs=cs, contcheck=cont, outlets=outlets, **sz),
+                                   port.dinftranslimaccum(ang, v["q"], v["tc"], cs=cs, contcheck=cont, outlets=outlets, **sz), ("tla", "tdep", "ctpt")):
+                    if r is not None:
+                        assert_bits(o, r, f"{n} (algebra {alg}) {tag}")
+    if {4, 5, 6} & set(algs):
+        for kw in ({}, {"mask": v["mask"], "thresh": thresh}):
+            for o, r, n in zip(td.gridnet_grid(p, outlets=outlets, **kw, **sz), port.gridnet(p, outlets=outlets, **kw, **sz), ("plen", "tlen", "gord")):
+                assert_bits(o, r, f"{n} {sorted(kw)} {what}")
+
+
+def _flow(dem, dx, dy):
+    fel = port.pitremove(dem)
+    return port.d8flowdir(fel, dx=dx, dy=dy)[0], port.dinfflowdir(fel, dx=dx, dy=dy)[0]
+
+
+def test_sibling_edge_shapes_against_c_restatement():
+    """The nine algebras on the degenerate shapes of test_edge_shapes_against_c_restatement (a single row / column, 2 and 3 rows,
+    widths that are not multiples of the tile, all nodata, a nodata ring, a constant grid), dx != dy, with and without -nc."""
+    rng = np.random.default_rng(14)
+    shapes = [(1, 9), (9, 1), (2, 5), (3, 3), (3, 70), (33, 65), (64, 129), (31, 257)]
+    grids = [(rng.random(s) * 50).astype(np.float32) for s in shapes]
+    ring = (rng.random((40, 37)) * 30).astype(np.float32); ring[0, :] = ring[-1, :] = ring[:, 0] = ring[:, -1] = -9999.0
+    grids += [np.full((12, 19), -9999.0, np.float32), ring, np.full((20, 21), 7.0, np.float32)]
+    for dem in grids:
+        p, ang = _flow(dem, 10.0, 12.0)
+        _check_siblings(p, ang, _sibling_values(rng, dem.shape), f"{dem.shape}", dx=10.0, dy=12.0)
+
+
+def test_siblings_with_many_tile_crossings(crossings):
+    """The nine algebras on the 2100 x 3000 DEM of test_sweep_with_many_tile_crossings_matches_the_reference (6 200 tiles, rivers across
+    hundreds of them: the warp-cooperative tail of algebras 1-6, algebra 9's second travelling value in global memory), with weights,
+    mask + threshold and the supply concentration; the case is checked to reach long rivers and mostly data cells."""
+    fel, p, sd8, ang = crossings
+    rng = np.random.default_rng(19)
+    shape = p.shape
+    sa = np.where(sd8 < 0, np.float32(0.0), sd8).astype(np.float32)
+    dm = rng.uniform(0.995, 1.0, shape).astype(np.float32); dm[rng.random(shape) < 1e-5] = -9999.0
+    w = rng.uniform(0.0, 2.0, shape).astype(np.float32)
+    q = rng.uniform(0.5, 3.0, shape).astype(np.float32)
+    tc = rng.uniform(0.0, 400.0, shape).astype(np.float32)
+    cs = rng.uniform(0.0, 2.0, shape).astype(np.float32)
+    dg = (rng.random(shape) < 0.001).astype(np.int16)
+    assert_bits(td.d8flowpathextremeup_grid(p, sa), port.d8flowpathextremeup(p, sa), "ssa max")
+    assert_bits(td.d8flowpathextremeup_grid(p, fel, usemax=False, contcheck=False), port.d8flowpathextremeup(p, fel, usemax=False, contcheck=False), "ssa min -nc")
+    gn = td.gridnet_grid(p)
+    for o, r, n in zip(gn, port.gridnet(p), ("plen", "tlen", "gord")):
+        assert_bits(o, r, n)
+    mask = np.minimum(gn[2].astype(np.int32), 3)              # Strahler order as the mask: the threshold cuts the first-order cells off
+    for o, r, n in zip(td.gridnet_grid(p, mask=mask, thresh=2), port.gridnet(p, mask=mask, thresh=2), ("plen", "tlen", "gord")):
+        assert_bits(o, r, n + " -mask -thresh 2")
+    dsca = td.dinfdecayaccum_grid(ang, dm)
+    assert_bits(dsca, port.dinfdecayaccum(ang, dm), "dsca")
+    assert_bits(td.dinfdecayaccum_grid(ang, dm, weights=w, contcheck=False), port.dinfdecayaccum(ang, dm, weights=w, contcheck=False), "dsca -wg -nc")
+    assert_bits(td.dinfconclimaccum_grid(ang, dm, q, dg, csol=2.0), port.dinfconclimaccum(ang, dm, q, dg, csol=2.0), "ctpt")
+    for cs_, cont in ((None, True), (cs, False)):
+        ours, ref = td.dinftranslimaccum_grid(ang, q, tc, cs=cs_, contcheck=cont), port.dinftranslimaccum(ang, q, tc, cs=cs_, contcheck=cont)
+        for o, r, n in zip(ours, ref, ("tla", "tdep", "ctpt")):
+            if r is not None:
+                assert_bits(o, r, f"{n} cs={cs_ is not None} contcheck={cont}")
+    assert gn[0].max() > 3e4 and gn[1].max() > 1e6 and gn[2].max() >= 5        # rivers of more than 1000 cells, thousands of tiles
+    assert dsca.max() > 1e6
+    assert (ours[0] != MISSINGFLOAT).mean() > 0.5 and (ours[1] > 0).mean() > 0.02 and (ours[2] > 0).mean() > 0.5
+
+
+def test_sibling_dinf_angle_torture():
+    """Algebras 3, 7, 8 and 9 on angles at and next to every place where prop() changes its mind (util.angle_torture), square and oblong
+    cells, with and without -nc."""
+    from util import angle_torture
+    rng = np.random.default_rng(21)
+    for dx, dy in ((30.0, 30.0), (12.5, 40.0)):
+        ang = angle_torture(ny=200, nx=330, dx=dx, dy=dy)
+        _check_siblings(None, ang, _sibling_values(rng, ang.shape), f"angle torture {dx}x{dy}", dx=dx, dy=dy, algs=(3, 7, 8, 9))
+
+
+def test_sibling_per_row_cell_sizes(tmp_path):
+    """Per-row (geographic) cell sizes: the non-uniform prop() branch of the D-infinity algebras and gridnet's per-row distances.  Grid
+    level with dxc / dyc of a geographic file; file level: each sibling executable on geographic files against the restatement with the
+    file's cell sizes."""
+    import ctypes
+    import os
+    dem = synth.punch_holes(synth.gen_dem(150, 210, hurst=0.8, tilt=1.0, seed=12))
+    geo = str(tmp_path / "geo.tif")
+    write_geographic_dem(geo, dem)
+    ny = dem.shape[0]
+    dxc, dyc = np.zeros(ny), np.zeros(ny)
+    assert td.lib().td_raster_cell_sizes(geo.encode(), dxc.ctypes.data_as(ctypes.c_void_p), dyc.ctypes.data_as(ctypes.c_void_p), ny) == 0
+    assert np.unique(dxc).size > 100 and np.unique(dyc).size > 1
+    fel = port.pitremove(dem)
+    p, _ = port.d8flowdir(fel, dx=dxc, dy=dyc)
+    ang, _ = port.dinfflowdir(fel, dx=dxc, dy=dyc)
+    rng = np.random.default_rng(22)
+    v = _sibling_values(rng, dem.shape)
+    v["dm"] = rng.uniform(0.2, 1.0, dem.shape).astype(np.float32)
+    _check_siblings(p, ang, v, "geographic", dxc=dxc, dyc=dyc, algs=(3, 4, 5, 6, 7, 8, 9))
+    # file level
+    q = lambda n: str(tmp_path / n)
+    for name, a, nd in (("p", p, -32768), ("ang", ang, ANG_ND), ("sa", v["sa"], -9999.0), ("dm", v["dm"], -9999.0), ("w", v["w"], -9999.0),
+                        ("q", v["q"], -9999.0), ("dg", v["dg"], -32768), ("tc", v["tc"], -9999.0), ("cs", v["cs"], -9999.0)):
+        td.write_raster(q(name + ".tif"), a, nd, like=geo)
+    assert td.raster_info(q("ang.tif"))["is_geographic"]
+    _run("d8flowpathextremeup", "-p", q("p.tif"), "-sa", q("sa.tif"), "-ssa", q("ssa.tif"), "-min")
+    assert_bits(td.read_raster(q("ssa.tif")), port.d8flowpathextremeup(p, v["sa"], usemax=False), "ssa -min (geographic file)")
+    _run("gridnet", "-p", q("p.tif"), "-plen", q("plen.tif"), "-tlen", q("tlen.tif"), "-gord", q("gord.tif"))
+    for n, r in zip(("plen", "tlen", "gord"), port.gridnet(p, dxc=dxc, dyc=dyc)):
+        assert_bits(td.read_raster(q(n + ".tif"), r.dtype), r, n + " (geographic file)")
+    _run("dinfdecayaccum", "-ang", q("ang.tif"), "-dm", q("dm.tif"), "-dsca", q("dsca.tif"))
+    assert_bits(td.read_raster(q("dsca.tif")), port.dinfdecayaccum(ang, v["dm"], dxc=dxc, dyc=dyc), "dsca (geographic file)")
+    _run("dinfdecayaccum", "-ang", q("ang.tif"), "-dm", q("dm.tif"), "-wg", q("w.tif"), "-nc", "-dsca", q("dscaw.tif"))
+    assert_bits(td.read_raster(q("dscaw.tif")), port.dinfdecayaccum(ang, v["dm"], weights=v["w"], contcheck=False, dxc=dxc, dyc=dyc), "dsca -wg -nc (geographic file)")
+    _run("dinfconclimaccum", "-ang", q("ang.tif"), "-dm", q("dm.tif"), "-q", q("q.tif"), "-dg", q("dg.tif"), "-ctpt", q("ctpt.tif"), "-csol", "1.5")
+    assert_bits(td.read_raster(q("ctpt.tif")), port.dinfconclimaccum(ang, v["dm"], v["q"], v["dg"], csol=1.5, dxc=dxc, dyc=dyc), "ctpt (geographic file)")
+    _run("dinftranslimaccum", "-ang", q("ang.tif"), "-tsup", q("q.tif"), "-tc", q("tc.tif"), "-cs", q("cs.tif"), "-tla", q("tla.tif"), "-tdep", q("tdep.tif"),
+         "-ctpt", q("ctptout.tif"))
+    for n, r in zip(("tla", "tdep", "ctptout"), port.dinftranslimaccum(ang, v["q"], v["tc"], cs=v["cs"], dxc=dxc, dyc=dyc)):
+        assert_bits(td.read_raster(q(n + ".tif")), r, n + " (geographic file)")
+
+
+def test_sibling_algebra_edges():
+    """The values where each algebra could take a wrong branch: sa ties and negative values (max and min), Strahler ties (three
+    tributaries of equal order), mask cells exactly at the threshold and masked-out cells in the middle of rivers, unresolved flats
+    (p = 0, angle -1: dependencies only), odd direction codes, dm = 0 / nodata, q <= 0 / nodata, dg on cells that receive flow, tc = 0,
+    cs nodata, and outlets: nested and disjoint basins, one off the grid, one on a nodata cell, none at all."""
+    rng = np.random.default_rng(31)
+    dem = synth.punch_holes(synth.gen_dem(130, 170, hurst=0.8, tilt=1.0, seed=33))
+    fel = port.pitremove(dem)
+    p, _ = port.d8flowdir(fel, dx=20.0, dy=25.0)
+    ang, _ = port.dinfflowdir(fel, dx=20.0, dy=25.0)
+    v = _sibling_values(rng, p.shape)
+    v["sa"] = rng.integers(-3, 3, p.shape).astype(np.float32)                 # ties everywhere, negative values
+    for k in ("dm", "q", "tc"):
+        v[k][rng.random(p.shape) < 0.05] = 0.0
+    v["q"][rng.random(p.shape) < 0.03] = -2.0
+    ad8 = port.aread8(p, contcheck=False)
+    mask = np.where(ad8 >= 0, ad8, 0).astype(np.int32)
+    river = (ad8 > 30) & (rng.random(p.shape) < 0.2)
+    mask[river] = 0                                                            # masked-out cells in the middle of rivers
+    v["mask"] = mask
+    assert (mask == 12).any()
+    _check_siblings(p, ang, v, "edge values", dx=20.0, dy=25.0, thresh=12)
+    # unresolved flats: direction 0 / angle -1
+    pf, _ = port.d8flowdir(fel, dx=20.0, dy=25.0, flats=False)
+    af, _ = port.dinfflowdir(fel, dx=20.0, dy=25.0, flats=False)
+    assert (pf == 0).sum() > 100 and (af == -1).sum() > 100
+    _check_siblings(pf, af, v, "flats", dx=20.0, dy=25.0, thresh=12)
+    # odd direction codes and another nodata value (algebras 1 and 2 follow the reference's aread8 quirks; gridnet the same graph)
+    po = rng.integers(-3, 13, size=p.shape).astype(np.int16)
+    po[rng.random(p.shape) < 0.05] = -1
+    for cont in (True, False):
+        for usemax in (True, False):
+            assert_bits(td.d8flowpathextremeup_grid(po, v["sa"], usemax=usemax, nodata=-1, contcheck=cont),
+                        port.d8flowpathextremeup(po, v["sa"], usemax=usemax, nodata=-1, contcheck=cont), f"ssa odd codes {usemax} {cont}")
+    for o, r, n in zip(td.gridnet_grid(po, nodata=-1, dx=20.0, dy=25.0), port.gridnet(po, nodata=-1, dx=20.0, dy=25.0), ("plen", "tlen", "gord")):
+        assert_bits(o, r, n + " odd codes")
+    # Strahler ties: three order-2 tributaries meet at (4, 4) (order 3), which drains south out of the grid
+    s = np.full((9, 9), -32768, np.int16)
+    for (r, c), d in {(2, 3): 8, (2, 5): 6, (3, 4): 7, (3, 2): 8, (5, 2): 2, (4, 3): 1, (3, 6): 6, (5, 6): 4, (4, 5): 5, (4, 4): 7, (5, 4): 7, (6, 4): 7,
+                      (7, 4): 7}.items():
+        s[r, c] = d
+    gord = td.gridnet_grid(s)[2]
+    assert gord[4, 4] == 3 and gord[3, 4] == gord[4, 3] == gord[4, 5] == 2
+    for o, r, n in zip(td.gridnet_grid(s), port.gridnet(s), ("plen", "tlen", "gord")):
+        assert_bits(o, r, n + " Strahler ties")
+    # outlets: nested (the 2nd lies upstream of the 1st), disjoint, off the grid, on a nodata cell; and none
+    ny, nx = p.shape
+    order = np.argsort(ad8.ravel())
+    top = int(order[-1])
+    up = next(int(c) for c in order[::-1][1:] if ad8.flat[c] < ad8.flat[top] and ad8.flat[c] > 20 and abs(c % nx - top % nx) + abs(c // nx - top // nx) < 40)
+    nodata_cell = int(np.flatnonzero(p.ravel() == -32768)[len(np.flatnonzero(p.ravel() == -32768)) // 2])
+    cells = [top, up, int(order[-300]), int(order[len(order) // 2]), nodata_cell]
+    outs = ([c % nx for c in cells] + [-4, nx + 3], [c // nx for c in cells] + [7, 2])
+    _check_siblings(p, ang, v, "outlets", dx=20.0, dy=25.0, outlets=outs, thresh=12)
+    _check_siblings(p, ang, v, "no outlets", dx=20.0, dy=25.0, outlets=([], []), contchecks=(True,), thresh=12)

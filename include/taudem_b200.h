@@ -43,6 +43,8 @@ extern "C" {
 #define TD_ERR_MISMATCH 5 /* companion raster mismatch (reference: MPI_Abort(MCW,5))    */
 #define TD_ERR_CUDA 90    /* CUDA runtime failure / no device                           */
 #define TD_ERR_ALLOC 91   /* device or host allocation failure (reference: -999)        */
+#define TD_ERR_FLAT_PASSES 92 /* a flat needs >= 32767 fall or rise passes: the reference's
+                                 16-bit pass counter wraps there (DESIGN.md §2)            */
 
 /* ---- version / diagnostics -------------------------------------------------------- */
 const char* td_version(void);            /* "5.4.0-b200" (TDVERSION, src/commonLib.h:63)  */

@@ -21,6 +21,7 @@ def lib():
         _lib = C.CDLL(_SO)
         _lib.orc_flood.argtypes = [_P, _P, _P, _I, _I, _F, _I]
         _lib.orc_set_skip_flats.argtypes = [_I]
+        _lib.orc_flat_stats.argtypes = [_P]
         _lib.orc_set_outlets.argtypes = [_P, _P, _I]
         _lib.orc_d8.argtypes = [_P, _P, _P, _I, _I, _F, _P, _P]
         _lib.orc_dinf.argtypes = [_P, _P, _P, _I, _I, _F, _P, _P]
@@ -69,6 +70,18 @@ def dinfflowdir(fel, nodata=-3.0e38, dx=30.0, dy=30.0, flats=True):
     dxc, dyc = _rows(dx, ny), _rows(dy, ny)
     assert lib().orc_dinf(_p(fel), _p(ang), _p(slp), nx, ny, nodata, _p(dxc), _p(dyc)) == 0
     return ang, slp
+
+
+FLAT_STATS = ("iters", "T", "U", "pits", "fall_level", "rise_level", "elev2")
+
+
+def flat_stats():
+    """What the last d8flowdir / dinfflowdir call's flat resolution reached: iters = outer iterations, T / U = the largest number
+    of fall / rise passes, pits = cells marked as pits, fall_level / rise_level = the largest number of cells that stop at one
+    fall level / are first marked in one rise pass, elev2 = the largest level + s before it is stored in 16 bits."""
+    out = np.zeros(len(FLAT_STATS), np.int64)
+    lib().orc_flat_stats(_p(out))
+    return dict(zip(FLAT_STATS, (int(v) for v in out)))
 
 
 class _Outlets:

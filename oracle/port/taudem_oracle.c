@@ -209,13 +209,24 @@ static void set2_flat(flatctx* f, const int16_t* elev2, const int16_t* dn, int J
   }
 }
 
+/* test hook: what the last d8flowdir / dinfflowdir call's flat resolution reached (orc_flat_stats) */
+static struct {
+  long iters;          /* outer iterations (resolve_once calls) */
+  long T, U;           /* largest number of fall / rise passes */
+  long pits;           /* flat cells marked as pits */
+  long fall_lev, rise_lev;   /* largest number of cells that stop at one fall level / are first marked in one rise pass */
+  long elev2;          /* largest level + s before it is stored in 16 bits */
+} g_fs;
+#define MAXL(a, b) if ((b) > (a)) (a) = (b)
+
 static long resolve_once(flatctx* f, int32_t* q, long nflat) {
   const int nx = f->nx, ny = f->ny;
   const size_t n = (size_t)nx * ny;
   int16_t* elev2 = (int16_t*)malloc(n * 2); int16_t* dn = (int16_t*)calloc(n, 2); int16_t* s = (int16_t*)calloc(n, 2);
   for (size_t c = 0; c < n; c++) elev2[c] = 1;
-  /* incfall: src/d8.cpp:509-558 */
-  long inc_old = -1, inc = 0; int st = 1;
+  g_fs.iters++;
+  /* incfall: src/d8.cpp:509-558; the pass counter is a short, as there */
+  long inc_old = -1, inc = 0, prev = nflat, passes = 0; short st = 1;
   while (inc != inc_old) {
     inc_old = inc; inc = 0;
     for (long q0 = 0; q0 < nflat; q0++) {
@@ -223,14 +234,18 @@ static long resolve_once(flatctx* f, int32_t* q, long nflat) {
       if (still_rising(f, elev2, i, j, st)) { elev2[q[q0]]++; inc++; }
     }
     st++;
+    passes++;
+    MAXL(g_fs.fall_lev, prev - inc);      /* the cells that stopped at this pass's level */
+    prev = inc;
   }
+  MAXL(g_fs.T, passes);
   if (inc > 0)   /* pits: src/d8.cpp:559-593 */
     for (long q0 = 0; q0 < nflat; q0++) {
       const int i = q[q0] % nx, j = q[q0] / nx;
-      if (still_rising(f, elev2, i, j, st)) { if (f->dinf) f->ang[q[q0]] = MISSINGFLOAT; else f->dir8[q[q0]] = MISSINGSHORT; }
+      if (still_rising(f, elev2, i, j, st)) { if (f->dinf) f->ang[q[q0]] = MISSINGFLOAT; else f->dir8[q[q0]] = MISSINGSHORT; g_fs.pits++; }
     }
   /* incrise: src/d8.cpp:595-638 */
-  long marked_old = 0;
+  long marked_old = 0, rpasses = 0;
   for (;;) {
     for (long q0 = 0; q0 < nflat; q0++) {
       const int i = q[q0] % nx, j = q[q0] / nx;
@@ -242,10 +257,16 @@ static long resolve_once(flatctx* f, int32_t* q, long nflat) {
     }
     long marked = 0;
     for (size_t c = 0; c < n; c++) if (dn[c] > 0) { s[c]++; marked++; }
+    rpasses++;
+    MAXL(g_fs.rise_lev, marked - marked_old);
     if (marked == marked_old) break;
     marked_old = marked;
   }
-  for (long q0 = 0; q0 < nflat; q0++) elev2[q[q0]] = (int16_t)(elev2[q[q0]] + s[q[q0]]);
+  MAXL(g_fs.U, rpasses);
+  for (long q0 = 0; q0 < nflat; q0++) {
+    MAXL(g_fs.elev2, (long)elev2[q[q0]] + s[q[q0]]);
+    elev2[q[q0]] = (int16_t)(elev2[q[q0]] + s[q[q0]]);
+  }
   /* directions from the artificial surface; what is still flat stays in the queue */
   long left = 0;
   for (long q0 = 0; q0 < nflat; q0++) {
@@ -261,9 +282,15 @@ static long resolve_once(flatctx* f, int32_t* q, long nflat) {
 /* test hook: stop after the positive-slope stencil (the input state of the flat resolution) */
 static int g_skip_flats = 0;
 void orc_set_skip_flats(int v) { g_skip_flats = v; }
+/* out[7] = outer iterations, largest T, largest U, pits, largest fall level, largest rise level, largest level + s */
+void orc_flat_stats(long* out) {
+  const long v[7] = {g_fs.iters, g_fs.T, g_fs.U, g_fs.pits, g_fs.fall_lev, g_fs.rise_lev, g_fs.elev2};
+  memcpy(out, v, sizeof v);
+}
 
 static void resolve_flats(flatctx* f) {
   const int nx = f->nx, ny = f->ny;
+  memset(&g_fs, 0, sizeof g_fs);
   if (g_skip_flats) return;
   int32_t* q = (int32_t*)malloc(sizeof(int32_t) * (size_t)nx * ny);
   long nflat = 0;

@@ -38,6 +38,7 @@ namespace td {
 namespace {
 
 constexpr int UNASSIGNED = 0x7fffffff;
+constexpr int MAXPASS = 32767;          // fall / rise passes at which the reference's short pass counter wraps
 
 struct D8Pol {
   using DirT = short;
@@ -204,7 +205,8 @@ __global__ void __launch_bounds__(256) k_bfs_level(const long long* __restrict__
   }
 }
 
-// finalise elev2 = level (+T+1 for unreachable cells, which are marked as pits) + s
+// finalise elev2 = level (+T+1 for unreachable cells, which are marked as pits) + s, stored as the reference's 16-bit elev2:
+// level + s wraps to a negative value past 32767 (T, U < 32767 keep level and s themselves in range)
 template <class P>
 __global__ void k_combine(const long long* __restrict__ list, unsigned long long n, int* __restrict__ lev,
                           const int* __restrict__ mk, typename P::DirT* __restrict__ dir, int T, int U) {
@@ -215,7 +217,7 @@ __global__ void k_combine(const long long* __restrict__ list, unsigned long long
   if (l == UNASSIGNED) { l = 1 + T; dir[ci] = P::pit(); }    // src/d8.cpp:559-593
   const int m = mk[ci];
   if (m > 0) l += U - m + 1;                                   // src/d8.cpp:640-646
-  lev[ci] = l;
+  lev[ci] = (short)l;
 }
 
 // setFlow2 (src/d8.cpp:412-454)
@@ -527,6 +529,13 @@ int resolve_flats(td_ctx* ctx, float* elev, typename P::DirT* dir, const Strip& 
         if (nu == 0) { U = u; break; }
         lo = hi; hi = end; ++u;
       }
+    }
+    // The reference counts passes in a short (src/d8.cpp:514, src/dinf.cpp:655): from pass 32767 on its counter wraps and its
+    // elev2 no longer follows the gradients, so there is no result to reproduce.
+    if (T >= MAXPASS || U >= MAXPASS) {
+      set_error("flat resolution: a flat needs " + std::to_string(std::max(T, U)) + " " + (T >= MAXPASS ? "fall" : "rise") +
+                " passes; the reference's 16-bit pass counter allows at most 32766");
+      return TD_ERR_FLAT_PASSES;
     }
     // ---- combine, set directions, collect what is still flat
     if (n) { k_combine<P><<<nblk(n), 256, 0, st>>>(cur, n, lev, mk, dir, T, U); TD_LAUNCHED(); }

@@ -284,6 +284,60 @@ def test_c_restatement_reproduces_every_stored_sibling_output(refrun, tmp_path):
     assert len(keys) == sum(len(case(tmp_path)[1]) for case in sibling_cases.CASES) == 18
 
 
+def test_flat_cases_reach_their_regimes_and_replay_the_reference(refrun, tmp_path):
+    """Every reference call of the flat-resolution GPU tests (tests/flat_cases.py: deep lake, crowded pockets, multi-pass,
+    pits, edges, 16-bit wrap; D8 and D-infinity, square cells and dx != dy), recomputed by the restatement and matched to its
+    stored digest (one reference rank).  On every call port.flat_stats() must show what the case is there to reach.  The
+    count is asserted: a call that is not replayed fails here."""
+    import port
+    import reference
+    if not port.available():
+        pytest.skip("oracle/port not built")
+    import flat_cases
+    keys, ncalls = set(), 0
+    for name in flat_cases.CASES:
+        for dx, dy, tool, arg in flat_cases.calls(name):
+            R = refrun.RefPipeline(workdir=str(tmp_path), dx=dx, dy=dy, np_ranks=1)
+            before = set(reference.replayed)
+            out = getattr(R, tool)(arg)
+            new = set(reference.replayed) - before
+            assert len(new) <= 1 and all(reference.replayed[k] == tool for k in new), (name, tool)
+            keys.add(reference.call_key(tool, dx, dy, 1, (arg,), {}))
+            ncalls += 1
+            if tool == "pitremove":
+                continue
+            assert not flat_cases.reach(name, port.flat_stats()), (name, tool, dx, dy, port.flat_stats())
+            d = out[0]
+            nd = (d == -32768) if tool == "d8flowdir" else (d < -1e38)
+            if name == "wrap16":
+                # the reference stores A's far end as a negative elev2: exactly one corridor cell is left flat and becomes a pit
+                assert int(nd[5, 1:-1].sum()) == 1 and int(nd[1:-1, 1:-1].sum()) == 1, (tool, np.argwhere(nd[1:-1, 1:-1]) + 1)
+            else:
+                assert not ((d == 0) if tool == "d8flowdir" else (d == -1.0)).any(), (name, tool)     # no flat left unresolved
+    seed_edge, seed_nd = flat_cases.edge_features(flat_cases.edges()[1])
+    assert seed_edge > 100 and seed_nd > 100, (seed_edge, seed_nd)
+    assert all(reference.replayed.get(k) for k in keys)
+    assert len(keys) == ncalls == 28
+
+
+def test_c_restatement_matches_the_live_reference_on_flat_cases(tmp_path, monkeypatch):
+    """Where oracle/_ref is built: the restatement's flat resolution against the reference executables, live, on the small flat
+    cases (multi-pass, pits in flats, edges), D8 and D-infinity, both cell sizes."""
+    import port
+    import refrun
+    if not (refrun.available() and port.available()):
+        pytest.skip("oracle/_ref not built")
+    import flat_cases
+    monkeypatch.setattr(refrun, "INPUTS_ONLY", False)
+    for name in ("multipass", "pits", "edges"):
+        _, fel = flat_cases.CASES[name]()
+        for dx, dy in flat_cases.SIZES:
+            R = refrun.RefPipeline(workdir=str(tmp_path), dx=dx, dy=dy)
+            for o, r, n in zip(port.d8flowdir(fel, dx=dx, dy=dy) + port.dinfflowdir(fel, dx=dx, dy=dy), R.d8flowdir(fel) + R.dinfflowdir(fel),
+                               ("p", "sd8", "ang", "slp")):
+                assert_bits(o, r, f"{name} {n} {dx}x{dy}")
+
+
 def _random_sibling_grids(rng, ny, nx):
     """A D8 grid (codes 0..8, flats unresolved, nodata border and holes) and a D-infinity angle grid (flats, nodata, arbitrary angles)
     of a random DEM, and value grids with nodata, zero and negative values"""

@@ -6,6 +6,7 @@ Bar: bit-exact fel, p, sd8, slp, ad8; <= 1e-5 relative (identical nodata masks) 
 import numpy as np
 import pytest
 
+import flat_cases
 import port
 import sibling_cases
 import taudem_b200 as td
@@ -819,3 +820,105 @@ def test_sibling_algebra_edges():
     outs = ([c % nx for c in cells] + [-4, nx + 3], [c // nx for c in cells] + [7, 2])
     _check_siblings(p, ang, v, "outlets", dx=20.0, dy=25.0, outlets=outs, thresh=12)
     _check_siblings(p, ang, v, "no outlets", dx=20.0, dy=25.0, outlets=([], []), contchecks=(True,), thresh=12)
+
+
+# ---------------------------------------------------------------- flat resolution (taudem_b200/csrc/flats.cu) at deep, crowded and multi-pass flats
+def _bfs_grid_threads():
+    """threads of one pass of k_bfs_level's fixed grid: SMs x 4 blocks x 256"""
+    import torch
+    return torch.cuda.get_device_properties(0).multi_processor_count * 4 * 256
+
+
+@pytest.mark.parametrize("name", list(flat_cases.CASES))
+def test_flat_cases_against_the_reference(refrun, tmp_path, name):
+    """Each flat case (tests/flat_cases.py) through d8flowdir_grid / dinfflowdir_grid against the reference (its stored outputs,
+    recomputed by the restatement), square cells and dx != dy: p, sd8, slp bit for bit, ang within the bar.  port.flat_stats()
+    of every reference call shows that the case reaches what it claims; for the pockets, a BFS level larger than one pass of the
+    fixed BFS grid on this device."""
+    dem, fel = flat_cases.CASES[name]()
+    for dx, dy, tool, arg in flat_cases.calls(name):
+        R = refrun.RefPipeline(workdir=str(tmp_path), dx=dx, dy=dy, np_ranks=1)
+        if tool == "pitremove":
+            assert_bits(td.pitremove_grid(dem), R.pitremove(dem), "fel")
+            continue
+        ref = getattr(R, tool)(fel)
+        stats = port.flat_stats()
+        assert not flat_cases.reach(name, stats), stats
+        if name == "pockets":
+            assert stats["rise_level"] > _bfs_grid_threads(), stats
+        what = f"{name} {dx}x{dy}"
+        if tool == "d8flowdir":
+            p, sd8 = td.d8flowdir_grid(fel, dx=dx, dy=dy)
+            assert_bits(sd8, ref[1], f"sd8 {what}"); assert_bits(p, ref[0], f"p {what}")
+        else:
+            ang, slp = td.dinfflowdir_grid(fel, dx=dx, dy=dy)
+            assert_bits(slp, ref[1], f"slp {what}"); assert_float_parity(ang, ref[0], f"ang {what}")
+
+
+@pytest.mark.parametrize("name", ["deep_lake", "pockets"])
+def test_flat_resolution_level_batches(name, monkeypatch):
+    """TAUDEM_B200_FLATS_BATCH = 0 (one launch and read-back per BFS level), 1, 3, 64 (the default) and 4096 levels per host read-back
+    on the deep lake (508 fall levels: 8 batches of 64) and the pockets (a level larger than one pass of the fixed grid): every
+    result bit-identical to the restatement.  The variable is read on every call."""
+    _, fel = flat_cases.CASES[name]()
+    dx, dy = flat_cases.SIZES[1]
+    p_o, sd8_o = port.d8flowdir(fel, dx=dx, dy=dy)
+    ang_o, slp_o = port.dinfflowdir(fel, dx=dx, dy=dy)
+    for batch in (0, 1, 3, 64, 4096):
+        monkeypatch.setenv("TAUDEM_B200_FLATS_BATCH", str(batch))
+        p, sd8 = td.d8flowdir_grid(fel, dx=dx, dy=dy)
+        assert_bits(p, p_o, f"p, batch {batch}"); assert_bits(sd8, sd8_o, f"sd8, batch {batch}")
+        ang, slp = td.dinfflowdir_grid(fel, dx=dx, dy=dy)
+        assert_bits(ang, ang_o, f"ang, batch {batch}"); assert_bits(slp, slp_o, f"slp, batch {batch}")
+
+
+@pytest.mark.parametrize("name", ["deep_lake", "pockets"])
+def test_flat_resolution_on_row_strips(name, tmp_path):
+    """TAUDEM_B200_GPUS=2 and 3 pitremove -> d8flowdir / dinfflowdir on files (k_merge: BFS levels that cross the strip boundaries,
+    which run through the lake and through rows of pockets): every file bit-identical to the one-GPU run, and p / ang to the
+    restatement."""
+    import os
+    import subprocess
+    dem, _ = flat_cases.CASES[name]()
+    dx, dy = flat_cases.SIZES[1]
+    d = tmp_path
+    td.write_raster(str(d / "dem.tif"), dem, -9999.0, dx=dx, dy=dy)
+
+    def run(gpus, tool, *args):
+        env = dict(os.environ, TAUDEM_B200_GPUS=str(gpus))
+        r = subprocess.run([_bin(tool)] + [str(a) for a in args], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env, timeout=600)
+        assert r.returncode == 0 and "error" not in r.stdout.lower(), r.stdout
+
+    for n in (1, 2, 3):
+        run(n, "pitremove", "-z", d / "dem.tif", "-fel", d / f"fel_{n}.tif")
+        run(n, "d8flowdir", "-fel", d / f"fel_{n}.tif", "-p", d / f"p_{n}.tif", "-sd8", d / f"sd8_{n}.tif")
+        run(n, "dinfflowdir", "-fel", d / f"fel_{n}.tif", "-ang", d / f"ang_{n}.tif", "-slp", d / f"slp_{n}.tif")
+    for nm, dt in (("fel", np.float32), ("p", np.int16), ("sd8", np.float32), ("ang", np.float32), ("slp", np.float32)):
+        one = td.read_raster(str(d / f"{nm}_1.tif"), dt)
+        for n in (2, 3):
+            assert_bits(td.read_raster(str(d / f"{nm}_{n}.tif"), dt), one, f"{nm} on {n} ranks")
+    fel = td.read_raster(str(d / "fel_1.tif"))
+    assert_bits(fel, port.pitremove(dem), "fel")
+    p_o, sd8_o = port.d8flowdir(fel, dx=dx, dy=dy)
+    assert_bits(td.read_raster(str(d / "p_1.tif"), np.int16), p_o, "p"); assert_bits(td.read_raster(str(d / "sd8_1.tif")), sd8_o, "sd8")
+    ang_o, slp_o = port.dinfflowdir(fel, dx=dx, dy=dy)
+    assert_float_parity(td.read_raster(str(d / "ang_1.tif")), ang_o, "ang"); assert_bits(td.read_raster(str(d / "slp_1.tif")), slp_o, "slp")
+
+
+def test_flat_needing_32767_passes_is_an_error(tmp_path):
+    """A corridor of 32 768 cells needs 32 768 fall passes; the reference's 16-bit pass counter wraps at 32767, so there is no
+    result to reproduce: d8flowdir_grid / dinfflowdir_grid fail with TD_ERR_FLAT_PASSES and the executable prints its error line.
+    A corridor of 32 766 cells (32 766 fall passes, the most there can be) still resolves."""
+    import subprocess
+    _, fel = flat_cases.corridor(32768)
+    for f in (td.d8flowdir_grid, td.dinfflowdir_grid):
+        with pytest.raises(td.TaudemError) as e:
+            f(fel)
+        assert e.value.code == 92 and "32768 fall passes" in str(e.value), str(e.value)
+    td.write_raster(str(tmp_path / "c.tif"), fel, -9999.0)
+    r = subprocess.run([_bin("d8flowdir"), "-fel", tmp_path / "c.tif", "-p", tmp_path / "p.tif", "-sd8", tmp_path / "sd8.tif"],
+                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    assert "D8FlowDir device error" in r.stdout and "16-bit pass counter" in r.stdout, r.stdout
+    _, ok = flat_cases.corridor(32766)
+    p, _ = td.d8flowdir_grid(ok)
+    assert (p[2, 1:-1] == 1).all()

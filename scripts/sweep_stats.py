@@ -3,8 +3,10 @@
   TAUDEM_B200_TIMING=1 python scripts/sweep_stats.py [n=16384] [reps=2]
 
 With TAUDEM_B200_TIMING=1 the kernel records, per tile visit, the cycles lane 0 spent waiting for a ticket, loading,
-running the wavefront and writing back, the cells evaluated and the wavefront iterations.
-TAUDEM_B200_WORKERS=<n> (fewer workers per SM) and TAUDEM_B200_POLL=1 (plain nanosleep polling) are experiment knobs of the kernel."""
+running the wavefront and writing back, the cells evaluated and the wavefront iterations, and counts the visits of carried
+tiles (claimed by the worker that made them ready, without a ticket: their wait is zero).
+TAUDEM_B200_WORKERS=<n> (fewer workers per SM), TAUDEM_B200_POLL=1 (plain nanosleep polling) and TAUDEM_B200_EXP=16 (no carried
+tiles) are experiment knobs of the kernel."""
 import os
 import sys
 
@@ -42,7 +44,7 @@ def main():
         if os.environ.get("TAUDEM_B200_TIMING"):
             c = [T.l.td_ctx_counter(T.ctx, 24 + i) for i in range(8)]
             v = max(c[3], 1)
-            line += f"\n    visits {c[3]} ({c[3] / ((n + 31) // 32) ** 2:.2f} per tile); cycles per visit: wait {c[4]//v} load {c[5]//v} wavefront {c[6]//v} write-back {c[7]//v}"
+            line += f"\n    visits {c[3]} ({c[3] / ((n + 31) // 32) ** 2:.2f} per tile), carried {c[0]} ({100 * c[0] / v:.1f} %); cycles per visit: wait {c[4]//v} load {c[5]//v} wavefront {c[6]//v} write-back {c[7]//v}"
             line += f"; cells/visit {c[1] / v:.0f}, wavefront iterations/visit {c[2] / v:.1f}, cycles/iteration {c[6] / max(c[2], 1):.0f}"
         print(line, flush=True)
         del out

@@ -15,6 +15,8 @@
 //    written back (one fence), flow that leaves the tile is one global atomic per crossing, and the arrival that
 //    zeroes a count activates the owning tile (per-tile state idle / queued / running / running + dirty, so that a
 //    tile is never processed by two warps at once);
+//  * the carry: of the tiles a visit made ready, the one its last crossing reached (a river leaving the tile) is claimed
+//    by the same warp and visited next, without a trip through the ticket queue;
 //  * the kernel ends when no tile is queued or running.
 // Flow that crosses the strip boundary (one strip per GPU) is recorded in `halo` for the exchange rounds of the
 // row-strip driver (src/aread8.cpp:282-297, linearpart::addBorders).
@@ -44,6 +46,7 @@ constexpr int RS = TS + 4;                            // ring row stride: cell l
 constexpr int STKCAP = TD_WSTK;                       // fork stack entries per worker (D-infinity)
 constexpr unsigned NODE_VALID = 0x8000u, NODE_CON = 0x1000u;
 constexpr unsigned FULL = 0xffffffffu;
+constexpr int EXP_NO_CARRY = 16;                      // TAUDEM_B200_EXP bit: every activation goes through the ticket queue (no carried tiles)
 // The scheduler's words (WArgs::ctr, 8-byte words, one 128-byte line each).  The ticket queue is cut into up to MAXSH
 // independent shards (tile t belongs to shard t & (nsh - 1), worker w pops from shard w & (nsh - 1)): one queue's head /
 // tail / finished counters were the throughput limit of the whole sweep (three hot addresses, ~7 ns per atomic each).
@@ -115,8 +118,8 @@ struct WArgs {
   PropRow prop;            // D-infinity: the strip's prop() table (prop.uniform: every row has the same cell size dx0) — else per-row angles from `theta`
   double dx0;              // the cell size a cell's own area adds (src/areadinf.cpp:216)
   unsigned long long* ctr; // scheduler words (see MAXSH)
-  unsigned long long* stat;// [1] cells, [2] wavefront iterations, [3] visits, [4..7] cycle statistics (TAUDEM_B200_TIMING)
-  int stats, poll, exp;    // exp: experiment switches (TAUDEM_B200_EXP)
+  unsigned long long* stat;// [0] carried visits, [1] cells, [2] wavefront iterations, [3] visits, [4..7] cycle statistics (TAUDEM_B200_TIMING)
+  int stats, poll, exp;    // exp: experiment switches (TAUDEM_B200_EXP; EXP_NO_CARRY)
   // peer mode (one strip per GPU, the neighbours' buffers mapped over NVLink with CUDA IPC): no exchange rounds — a tile
   // delivers into the neighbour GPU exactly as it delivers into a neighbour tile.  Every GPU only WRITES remote memory
   // (the neighbour's halo-area buffer, counts, tile states, queue); everything it reads is its own.
@@ -305,10 +308,13 @@ __device__ int sched_pop(const WArgs& a, int q, bool scanner) {
 }
 // (every atomic of the visit has returned its result by now — the counts, the deliveries, the activations — and the plain
 //  stores were fenced before them: nothing of the visit is still in flight when the tile is released)
-__device__ void sched_finish(const WArgs& a, int t) {
+// A worker that popped a tile owes one `done` for that push.  A tile it carries (claimed at the end of a visit, never pushed)
+// adds nothing to the tails, so a visit that hands over to a carried tile does not pay: the chain of carried visits pays once,
+// when it ends.  Until then the shards stay unbalanced, so nobody can declare the end (nor, in peer mode, the strip passive).
+__device__ void sched_finish(const WArgs& a, int t, bool pay) {
   const bool sys = edge_tile(a, t);
   if (W_CAS_IF(sys, a.state + t, 2, 0) != 2) { W_EXCH_IF(sys, a.state + t, 1); sched_push(a, t); }
-  atomicAdd(w_done(a.ctr, t & (a.nsh - 1)), 1ull);
+  if (pay) atomicAdd(w_done(a.ctr, t & (a.nsh - 1)), 1ull);
 }
 
 // Zeroing by a kernel, not cudaMemsetAsync: memsets are executed by the copy engines, where they queue behind whatever
@@ -352,7 +358,7 @@ __global__ void k_wsched_init(int* state, int* tq, int ntiles, unsigned long lon
   }
   if (i == 0) {
     ctr[C_ACTIVE] = 1ull;
-    for (int j = 1; j < 8; ++j) stat[j] = 0;
+    for (int j = 0; j < 8; ++j) stat[j] = 0;
   }
 }
 
@@ -426,12 +432,16 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
     __syncthreads();
   }
 
+  int carry = -1;          // the tile this worker claimed at the end of its last visit (warp-uniform), else -1
   for (;;) {
     long long tk0 = 0, tk1 = 0, tk2 = 0, tk3 = 0;
-    int t = -1;
-    if (lane == 0) { if (a.stats) tk0 = clock64(); t = sched_pop(a, myq, wid == 0); if (a.stats) tk1 = clock64(); }
-    t = __shfl_sync(FULL, t, 0);
-    if (t < 0) return;
+    int t = carry;
+    if (t < 0) {
+      if (lane == 0) { if (a.stats) tk0 = clock64(); t = sched_pop(a, myq, wid == 0); if (a.stats) tk1 = clock64(); }
+      t = __shfl_sync(FULL, t, 0);
+      if (t < 0) return;
+    } else if (a.stats && lane == 0) { tk0 = clock64(); tk1 = tk0; }
+    carry = -1;
     const int ty = t / a.ntx, tx = t - ty * a.ntx;
     const int c0 = tx * TS, r0 = 1 + ty * TH;
 
@@ -851,8 +861,10 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
     }
     __syncwarp();
     if (a.exp & 8) fence_acq_rel(); else __threadfence();          // release by the lanes that publish: every lane's stores (ordered by the barrier) before their atomics
-    // flow that leaves the tile first (the neighbours wait for it), then the rim's counts
+    // flow that leaves the tile first (the neighbours wait for it), then the rim's counts.  Every lane holds back the last tile
+    // its crossings made ready (`pend`, crossing `pend_e`); the others it activates at once.
     const int ne = M.next;
+    int pend = -1, pend_e = -1;
     for (int e = lane; e < ne; e += 32) {
       const int l = M.ext[e] & 0x7ff, k = (M.ext[e] >> 11) + 1;
       const int lr = l >> 5, lx = l & 31;
@@ -868,7 +880,30 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
       const long long ci = s.idx(r, c);
       const unsigned sh = (unsigned)(ci & 3) * 8u;
       const unsigned old = W_ADD_IF(a.peer && (r == 1 || r == s.ny), a.cntw + (ci >> 2), 0u - (1u << sh));
-      if (((old >> sh) & 0xffu) == 1u) sched_activate(a, ((r - 1) / TH) * a.ntx + c / TS);
+      if (((old >> sh) & 0xffu) == 1u) {
+        if (pend >= 0) sched_activate(a, pend);
+        pend = ((r - 1) / TH) * a.ntx + c / TS; pend_e = e;
+      }
+    }
+    // The carry: of the tiles of this strip made ready by a crossing, the one of the LAST crossing made (normally the river
+    // that the one-chain mode followed to the tile's edge) is visited next by this worker, without the ticket queue: claimed
+    // idle -> running here, it skips the push, the pop, a waiting worker's back-off and the queue behind other tiles.  A tile
+    // that is queued or running already (or every tile, with EXP_NO_CARRY) is activated as before.
+    int hi = pend_e;
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) hi = max(hi, __shfl_xor_sync(FULL, hi, d));
+    if (hi >= 0) {
+      const int wl = hi & 31;                               // crossing e was delivered by lane e % 32
+      const int ct = __shfl_sync(FULL, pend, wl);
+      if (lane == wl) {
+        // the claim's result is consumed (the branch) before the carried visit loads the tile's counts, so those loads cannot
+        // be issued before the claim was performed: whoever delivers into the tile after it re-activates it (2 -> 3)
+        if (!(a.exp & EXP_NO_CARRY) && W_CAS_IF(edge_tile(a, ct), a.state + ct, 0, 2) == 0) {
+          carry = ct;
+          if (a.stats) atomicAdd(a.stat, 1ull);
+        } else sched_activate(a, ct);
+      } else if (pend >= 0 && pend != ct) sched_activate(a, pend);   // (the claim or the activation of `ct` covers a lane's own `ct`)
+      carry = __shfl_sync(FULL, carry, wl);
     }
 #pragma unroll
     for (int rp = 0; rp < RPL; ++rp) {
@@ -887,7 +922,7 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
     __syncwarp();
     if (lane == 0) {
       if (M.dirty) sched_activate(a, t);
-      sched_finish(a, t);
+      sched_finish(a, t, carry < 0);
     }
     if (a.stats) {
       int ncell = 0;

@@ -50,9 +50,13 @@ __device__ __noinline__ void d8_literal(const float* q, int sw, double fE, doubl
 // member inside that band; if it is not the largest drop itself the cell is ambiguous (two nearly equal
 // drops, rare) and takes the literal eight-product path.  A group whose largest drop is <= 0 has no
 // member inside the band and can never win (S > 0 is required), so it never raises the flag.
+// The band argument holds while S and the largest drop of every group that attains it are normal floats (a drop
+// 2^-20 lower then lies at least 7 ulps lower, and m * (1 - 2^-20) is computed to 2^-24).  smin = 2^-125 max(1, fE, fN)
+// (the row's) makes S >= smin imply both; a cell whose S is below smin (subnormal drops or slopes) or infinite (the
+// product overflows float: every overflowing drop rounds to the same slope) takes the literal path, as do ambiguous ones.
 // One cell from its eight drops e_k = z - z_k.
 __device__ __forceinline__ bool d8_pick(float e1, float e2, float e3, float e4, float e5, float e6, float e7, float e8, double fE, double fN,
-                                        double fD, int& dir, float& smax) {
+                                        double fD, float smin, int& dir, float& smax) {
   const float m15 = fmaxf(e1, e5), m37 = fmaxf(e3, e7), mD = fmaxf(fmaxf(e2, e4), fmaxf(e6, e8));
   const float sE = (float)(fE * (double)m15), sN = (float)(fN * (double)m37), sD = (float)(fD * (double)mD);
   const float S = fmaxf(fmaxf(sE, sN), sD);
@@ -70,7 +74,8 @@ __device__ __forceinline__ bool d8_pick(float e1, float e2, float e3, float e4, 
   const bool pos = S > 0.f;
   dir = pos ? (best & 15) : 0;
   smax = pos ? S : 0.f;
-  return amb & pos;
+  const bool normal = (S >= smin) & (S <= FLT_MAX);
+  return (amb | !normal) & pos;
 }
 
 constexpr int STAGES = 3;
@@ -124,6 +129,7 @@ __global__ void __launch_bounds__(256) k_d8_stencil(const TD_GRID_CONSTANT TileM
         load_row(pm + (k + 2) * G::SW, rc, nc);
         const RowFact* rf = rowf + (r - 1);
         const double fE = rf->fE, fN = rf->fN, fD = rf->fD;
+        const float smin = 0x1p-125f * fmaxf(1.f, (float)fmax(fE, fN));     // d8_pick: the band argument holds for S >= smin
         float h[5], v[4], g[5], f[5];               // b[j]-b[j+1], b[j+1]-c[j+1], b[j]-c[j+1], b[j+1]-c[j]
 #pragma unroll
         for (int j = 0; j < 5; ++j) { h[j] = rb[j] - rb[j + 1]; g[j] = rb[j] - rc[j + 1]; f[j] = rb[j + 1] - rc[j]; }
@@ -139,7 +145,7 @@ __global__ void __launch_bounds__(256) k_d8_stencil(const TD_GRID_CONSTANT TileM
           const bool bad = (fminf(fminf(colmin[i], colmin[i + 1]), colmin[i + 2]) < TD_MINEPS) || ((em >> i) & 1u);
           int d; float smax;
           // e1 = z - E, e2 = z - NE, e3 = z - N, e4 = z - NW, e5 = z - W, e6 = z - SW, e7 = z - S, e8 = z - SE
-          if (d8_pick(h[i + 1], -pf[i + 1], -pv[i], -pg[i], -h[i], f[i], v[i], g[i + 1], fE, fN, fD, d, smax))
+          if (d8_pick(h[i + 1], -pf[i + 1], -pv[i], -pg[i], -h[i], f[i], v[i], g[i + 1], fE, fN, fD, smin, d, smax))
             d8_literal(pm + (k + 1) * G::SW + i, G::SW, fE, fN, fD, &d, &smax);
           od[i] = bad ? TD_MISSINGSHORT : (short)d;
           os[i] = bad ? -1.0f : smax;

@@ -10,6 +10,10 @@
 //     the float error is ~1e-6, so every facet whose float rank is more than 4e-5 below the best one cannot be the
 //     exact winner.  In all but ~1e-4 of the cells exactly one facet survives: the winner is known without FP64.
 //     Cells with several survivors evaluate those facets in FP64 in increasing K with the reference's strict '>'.
+//     The 1e-6 bound holds while the largest squared slope is a finite float >= 2^-100: rounding in the subnormal range
+//     then costs at most a few 2^-149 absolutely, and no term has overflowed (an overflow makes the square infinite).
+//     Outside that range (relief far below or far above any terrain's, or neighbour differences that overflow float)
+//     the squares underflow to 0 or collapse onto +inf, so every facet with a positive slope is evaluated in FP64.
 //  2. the winner is evaluated ONCE per cell, uniformly over the warp (no per-facet divergence): both quotients,
 //     the clipped slope, the root, then selects; the three divisions are divisions by row constants
 //     (div_const, rowfact.cuh: five FMA-pipe FP64 operations each, correctly rounded), atan2 only for the facets whose
@@ -59,7 +63,8 @@ __device__ __forceinline__ void facet_geom(int K, int sw, int& o1, int& o2, bool
   d1x = (K == 1 || K == 4 || K == 5 || K == 8);
 }
 
-// several facets within the float error of the best one: the exact slopes decide (increasing K, strict '>'); rare, out of line
+// several facets within the float error of the best one, or every facet with a positive slope where the float ranking does not
+// hold: the exact slopes decide (increasing K, strict '>'); rare, out of line
 __device__ __noinline__ int exact_pick(const float* q0, int sw, unsigned cand, const RowFact* rfp) {
   const RowFact rf = *rfp;
   const double E0 = (double)q0[0];
@@ -138,16 +143,23 @@ __global__ void __launch_bounds__(256) k_dinf_stencil(const TD_GRID_CONSTANT Til
         const float thr = smaxf * 0.99996f;
 #pragma unroll
         for (int K = 1; K <= 8; ++K) cand |= (st[K - 1] >= thr && st[K - 1] > 0.f) ? (1u << (K - 1)) : 0u;
-        if (bad) cand = 0;
-        // two facets that share E1 and both have S2 < 0 have the same slope S1 bit for bit, two that share E2 and are both
-        // clipped have the same slope (E0 - E2) / DD: the lower K wins such a tie (strict '>'), no FP64 needed to say so
-        {
+        if (smaxf >= 0x1p-100f && smaxf <= FLT_MAX) {
+          // two facets that share E1 and both have S2 < 0 have the same slope S1 bit for bit, two that share E2 and are both
+          // clipped have the same slope (E0 - E2) / DD: the lower K wins such a tie (strict '>'), no FP64 needed to say so
           const unsigned A = cand & s2neg, B = cand & clipsafe;
           unsigned drop = ((A & 0x2au) << 1) & A;                         // pairs (2,3) (4,5) (6,7) share E1
           if ((A & 0x81u) == 0x81u) drop |= 0x80u;                        // pair (1,8)
           drop |= ((B & 0x55u) << 1) & B;                                 // pairs (1,2) (3,4) (5,6) (7,8) share E2
           cand &= ~drop;
+        } else {
+          // the float ranking is not reliable here (header, 1.): every facet with a positive slope, i.e. z above E1 or E2,
+          // goes to the FP64 evaluation, without the drop rules (their float tests are not reliable either)
+          cand = 0;
+#pragma unroll
+          for (int K = 1; K <= 8; ++K)
+            cand |= (z > nb[1 + fI1(K)][1 + fJ1(K)] || z > nb[1 + fI2(K)][1 + fJ2(K)]) ? (1u << (K - 1)) : 0u;
         }
+        if (bad) cand = 0;
         int KD = cand ? __ffs(cand) : 0;
         if (cand & (cand - 1u)) KD = exact_pick(q0, G::SW, cand, rfp);
         // ---- 2. the winner, once and uniformly

@@ -303,6 +303,49 @@ int td_aread8_sweep_run_dev(td_ctx*, const float* w, float* ad8, td_strip s, flo
 int td_area_sweep_run_dev(td_ctx*, const float* ang, const float* w, float* sca, td_strip s, int usew,
                           int contcheck, const double* dxc, int* halo_out, void* stream);
 
+/* The five sibling sweep tools on row strips, with the same protocol: the tool's *_deps_dev (it initialises the outputs to the
+ * tool's nodata), td_sweep_begin_dev, then rounds of the tool's *_sweep_run_dev(..., halo_out, ...) and td_sweep_apply_halo_dev;
+ * or peer mode (td_sweep_peer_export_dev with dinf = 0 for the D8 tools, 1 for the D-infinity ones, ..., td_sweep_peer_begin_dev,
+ * a barrier, one *_sweep_run_dev per rank).  Every round the caller exchanges, with the halo_out arrays, the first / last owned
+ * rows of the value the sweep carries (ssa, plen / tlen / the Strahler order, dsca, ctpt, tla) into the neighbours' halo rows.
+ * Inputs read at a neighbour cell need valid halo rows before the deps call (like p / ang): listed per tool.  D-infinity tools on
+ * rasters whose rows have different cell sizes call td_set_halo_cell_sizes_dev first.  dxc / dyc: DEVICE arrays of ny doubles.
+ *
+ * d8flowpathextremeup: halo rows of p.  ssa starts as MISSINGFLOAT; sa needs no halo rows.                                     */
+int td_d8flowpathextremeup_deps_dev(td_ctx*, const int16_t* p, float* ssa, td_strip s, int16_t p_nodata, void* stream);
+int td_d8flowpathextremeup_sweep_run_dev(td_ctx*, const float* sa, float* ssa, td_strip s, int usemax, int contcheck, int* halo_out,
+                                         void* stream);
+/* dinfdecayaccum: halo rows of ang and dm (w: owned rows only, NULL = no weights).  dsca starts as MISSINGFLOAT.                */
+int td_dinfdecayaccum_deps_dev(td_ctx*, const float* ang, float* dsca, td_strip s, float ang_nodata, const double* dxc,
+                               const double* dyc, void* stream);
+int td_dinfdecayaccum_sweep_run_dev(td_ctx*, const float* ang, const float* dm, const float* w, float* dsca, td_strip s,
+                                    float dm_nodata, int contcheck, const double* dxc, int* halo_out, void* stream);
+/* dinfconclimaccum: halo rows of ang, dm and q (dg: owned rows only).  ctpt starts as MISSINGFLOAT.                              */
+int td_dinfconclimaccum_deps_dev(td_ctx*, const float* ang, float* ctpt, td_strip s, float ang_nodata, const double* dxc,
+                                 const double* dyc, void* stream);
+int td_dinfconclimaccum_sweep_run_dev(td_ctx*, const float* ang, const float* dm, const float* q, const int16_t* dg, float* ctpt,
+                                      td_strip s, float dm_nodata, float q_nodata, float csol, int contcheck, const double* dxc,
+                                      int* halo_out, void* stream);
+/* dinftranslimaccum: halo rows of ang (tsup, tc, cs: owned rows only).  tla, tdep and ctpt start as MISSINGFLOAT.  With -cs
+ * (cs and ctpt given) the caller exchanges the first / last owned rows of ctpt every round too, together with those of tla.    */
+int td_dinftranslimaccum_deps_dev(td_ctx*, const float* ang, float* tla, float* tdep, float* ctpt /*NULL unless cs*/, td_strip s,
+                                  float ang_nodata, const double* dxc, const double* dyc, void* stream);
+int td_dinftranslimaccum_sweep_run_dev(td_ctx*, const float* ang, const float* tsup, const float* tc, const float* cs /*NULL or*/,
+                                       float* tla, float* tdep, float* ctpt /*with cs*/, td_strip s, float tsup_nodata, float tc_nodata,
+                                       float cs_nodata, int contcheck, const double* dxc, int* halo_out, void* stream);
+/* gridnet: three sweeps in turn (which = 0 longest path plen, 1 total path tlen, 2 Strahler order), each with its own
+ * td_gridnet_deps_dev + begin + rounds (or peer begin + barrier + run), then td_gridnet_order_dev turns the third sweep's floats
+ * into gord (int16, -1 = nodata).  Halo rows of p, and of the mask when there is one: td_gridnet_mask_dev turns it (int32, with
+ * halo rows) into the 0 / 1 grid `ok` (NULL = no mask) of the owned rows and the halo rows.  dist: DEVICE array of ny x 8 floats,
+ * dist[row][k - 1] = (float)sqrt(dxc^2 d1[k]^2 + dyc^2 d2[k]^2) of the strip's own rows (src/gridnet.cpp:190-200).  outlets = 1
+ * after td_sweep_restrict_dev (single strip).  Every sweep starts its output as -1.                                            */
+int td_gridnet_mask_dev(td_ctx*, const int32_t* mask, float* ok, td_strip s, int thresh, void* stream);
+int td_gridnet_deps_dev(td_ctx*, const int16_t* p, float* out, td_strip s, int16_t p_nodata, void* stream);
+int td_gridnet_sweep_run_dev(td_ctx*, int which, const float* ok /*NULL = no mask*/, const float* dist, float* out, td_strip s,
+                             int outlets, int* halo_out, void* stream);
+int td_gridnet_order_dev(td_ctx*, const float* order, const int16_t* p, const float* ok, int16_t* gord, td_strip s, int16_t p_nodata,
+                         int outlets, void* stream);
+
 /* point-wise consumers on device strips (pointwise.cu) */
 int td_threshold_dev(td_ctx*, const float* ssa, const float* mask, int16_t* src, td_strip s, float thresh, float ssa_nodata, void* stream);
 int td_twi_dev(td_ctx*, const float* slp, const float* sca, float* twi, td_strip s, float slp_nodata, float sca_nodata, void* stream);

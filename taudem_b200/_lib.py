@@ -106,6 +106,18 @@ SIGNATURES = {
     "td_sweep_peer_off_dev": (None, [_P]),
     "td_set_halo_cell_sizes_dev": (None, [_P, _D, _D, _D, _D]),
     "td_area_sweep_run_dev": (_I, [_P, _P, _P, _P, Strip, _I, _I, _P, _P, _P]),
+    "td_d8flowpathextremeup_deps_dev": (_I, [_P, _P, _P, Strip, C.c_int16, _P]),
+    "td_d8flowpathextremeup_sweep_run_dev": (_I, [_P, _P, _P, Strip, _I, _I, _P, _P]),
+    "td_dinfdecayaccum_deps_dev": (_I, [_P, _P, _P, Strip, _F, _P, _P, _P]),
+    "td_dinfdecayaccum_sweep_run_dev": (_I, [_P, _P, _P, _P, _P, Strip, _F, _I, _P, _P, _P]),
+    "td_dinfconclimaccum_deps_dev": (_I, [_P, _P, _P, Strip, _F, _P, _P, _P]),
+    "td_dinfconclimaccum_sweep_run_dev": (_I, [_P, _P, _P, _P, _P, _P, Strip, _F, _F, _F, _I, _P, _P, _P]),
+    "td_dinftranslimaccum_deps_dev": (_I, [_P, _P, _P, _P, _P, Strip, _F, _P, _P, _P]),
+    "td_dinftranslimaccum_sweep_run_dev": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, Strip, _F, _F, _F, _I, _P, _P, _P]),
+    "td_gridnet_mask_dev": (_I, [_P, _P, _P, Strip, _I, _P]),
+    "td_gridnet_deps_dev": (_I, [_P, _P, _P, Strip, C.c_int16, _P]),
+    "td_gridnet_sweep_run_dev": (_I, [_P, _I, _P, _P, _P, Strip, _I, _P, _P]),
+    "td_gridnet_order_dev": (_I, [_P, _P, _P, _P, _P, Strip, C.c_int16, _I, _P]),
 }
 
 

@@ -162,7 +162,29 @@ __global__ void __launch_bounds__(256) k_deps_d8(const TD_GRID_CONSTANT TileMap 
   }
 }
 
+// The node words of the halo rows (rows 0 / ny + 1 where a neighbour strip exists) hold only the direction code of the
+// neighbour's edge cell (0 for nodata and codes outside 0..8).  gridnet's algebras look at a contributor's code (a code 0
+// contributes nothing, src/gridnet.cpp:393); k_deps_d8 leaves these rows alone.
+__global__ void k_halo_codes_d8(const short* __restrict__ p, unsigned short* __restrict__ node, Strip s, short nodata) {
+  const int c = (int)(blockIdx.x * blockDim.x + threadIdx.x);
+  if (c >= s.pitch) return;
+#pragma unroll
+  for (int side = 0; side < 2; ++side) {
+    if (!(side == 0 ? s.has_top : s.has_bot)) continue;
+    const long long o = s.idx(side == 0 ? 0 : s.ny + 1, c);
+    const int d = p[o];
+    node[o] = (c < s.nx && d != (int)nodata && (unsigned)d <= 8u) ? (unsigned short)((unsigned)d << 8) : (unsigned short)0;
+  }
+}
+
 }  // namespace
+
+cudaError_t launch_halo_codes_d8(const short* p, unsigned short* node, const Strip& s, short nodata, cudaStream_t st) {
+  if (!s.has_top && !s.has_bot) return cudaSuccess;
+  k_halo_codes_d8<<<(s.pitch + 255) / 256, 256, 0, st>>>(p, node, s, nodata);
+  TD_LAUNCHED();
+  return cudaGetLastError();
+}
 
 cudaError_t launch_deps_d8(const short* p, unsigned short* node, unsigned char* cnt, float* area, const Strip& s, short nodata,
                            cudaStream_t st, float area_init) {

@@ -14,6 +14,7 @@ int resolve_flats_dinf(td_ctx* ctx, float* elev, float* ang, const Strip& s, con
                        const double* thA, const double* thB, long long* nleft, const td_strip_comm* comm, cudaStream_t st);
 cudaError_t launch_deps_d8(const short* p, unsigned short* node, unsigned char* cnt, float* area, const Strip& s,
                            short nodata, cudaStream_t st, float area_init = -1.0f);
+cudaError_t launch_halo_codes_d8(const short* p, unsigned short* node, const Strip& s, short nodata, cudaStream_t st);   // gridnet on row strips
 cudaError_t launch_deps_dinf(const float* ang, unsigned short* node, unsigned char* cnt, float* area, const Strip& s,
                              float nodata, const double* theta, cudaStream_t st, float area_init = -1.0f);
 cudaError_t zero_words(void* p, size_t bytes, cudaStream_t st);     // a multiple of 4 bytes, zeroed by a kernel (never by a copy engine)
@@ -48,6 +49,7 @@ int launch_twi(const float* slp, const float* sca, float* twi, const Strip& s, f
 int launch_mask_ok(const int* mask, float* ok, const Strip& s, int thresh, cudaStream_t st);
 int launch_gord_finish(const float* g, const short* p, const float* ok, const unsigned short* node, short* gord, const Strip& s, short p_nodata,
                        int outlets, cudaStream_t st);
+void gridnet_dist_table(const double* dxc, const double* dyc, int ny, float* dist);   // host: gridnet's per-row distances (capi.cu)
 cudaError_t launch_gen_dem(float* dem, const Strip& s, int row0, int total_ny, unsigned seed, float hurst, float tilt, cudaStream_t st);
 cudaError_t launch_gen_w(float* w, const Strip& s, int row0, unsigned seed, cudaStream_t st);
 }  // namespace td

@@ -1,4 +1,4 @@
-// Multi-GPU contributing area behind the file-level entry points (mgpu.cu): one forked process per GPU.
+// Multi-GPU sweeps and flow directions behind the file-level entry points (mgpu.cu): one forked process per GPU.
 #pragma once
 #include <stddef.h>
 
@@ -22,11 +22,30 @@ struct MgpuFlowJob {
   void* out0 = nullptr;
   float* out1 = nullptr;
 };
-int mgpu_world();                                  // TAUDEM_B200_GPUS (1 = the single-GPU path)
+// the five sibling sweep tools on row strips; in[] = the further inputs (NULL = not used) and out[] = the outputs (mappings from
+// mgpu_alloc_shared, nx * ny cells of the output's type) of each tool:
+//   EXTREMEUP  d8flowpathextremeup  in: sa                 out: ssa
+//   GRIDNET    gridnet              in: mask (int32)       out: plen, tlen, gord (int16)
+//   DECAY      dinfdecayaccum       in: dm, w              out: dsca
+//   CONCLIM    dinfconclimaccum     in: dm, q, dg (int16)  out: ctpt
+//   TRANSLIM   dinftranslimaccum    in: tsup, tc, cs       out: tla, tdep, ctpt (with cs)
+struct MgpuSibJob {
+  enum { EXTREMEUP = 0, GRIDNET, DECAY, CONCLIM, TRANSLIM };
+  int tool = EXTREMEUP;
+  const char* dirfile = nullptr;              // p (D8 tools) or ang
+  const char* in[3] = {nullptr, nullptr, nullptr};
+  int usemax = 1, contcheck = 1, thresh = 0;
+  float csol = 0.f;
+  int nx = 0, ny = 0;
+  void* out[3] = {nullptr, nullptr, nullptr};
+};
+int mgpu_world();                                // TAUDEM_B200_GPUS (1 = the single-GPU path)
 void* mgpu_alloc_shared(size_t bytes);             // anonymous shared mapping (visible to the forked ranks)
 void mgpu_free_shared(void* p, size_t bytes);
 // runs the job on `world` ranks; compute_seconds = the slowest rank's time from the dependency stencil to the end of the sweep
 int mgpu_area(const MgpuJob& job, int world, double* compute_seconds, int* rounds);
+// the same for a sibling sweep tool (rounds: summed over gridnet's three sweeps; 1 per sweep in peer mode)
+int mgpu_sibling(const MgpuSibJob& job, int world, double* compute_seconds, int* rounds);
 // rounds = relaxation / exchange rounds of pitremove, 0 for the flow directions; flats_left = unresolved flat cells of the whole grid
 int mgpu_flow(const MgpuFlowJob& job, int world, double* compute_seconds, int* rounds, long long* flats_left);
 }  // namespace td

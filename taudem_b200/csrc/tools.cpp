@@ -163,13 +163,51 @@ void nodata_msgs(double nd, const char* what, double cast) {
   printf("Nodata value input to create partition from file: %lf\n", nd);
   printf("Nodata value recast to %s used in partition raster: %s\n", what, std::to_string(cast).c_str());
 }
-// one more float (or int16) grid of a sibling tool: open, compare with the angle grid, read
+// one more grid of a sibling tool: open, compare with the direction grid (companion_open); then read it
+int companion_open(const Input& a, Input& g, const char* file, tdio::DType dt, const char* type, const char* what = "companion grid does not match") {
+  if (int rc = g.open(file)) return rc;
+  if (!tdio::compare_rasters(a.r, a.path, g.r, g.path)) { printf("File sizes do not match\n%s\n", file); td::set_error(what); return TD_ERR_MISMATCH; }
+  if (dt == tdio::DT_F32) nodata_msgs(g.r.nodata(), type, (float)g.r.nodata());
+  else if (dt == tdio::DT_I32) nodata_msgs(g.r.nodata(), type, (int32_t)g.r.nodata());
+  else nodata_msgs(g.r.nodata(), type, (int16_t)g.r.nodata());
+  return TD_OK;
+}
 template <typename T>
 int companion(Input& a, Input& g, const char* file, std::vector<T>* data, tdio::DType dt, const char* type) {
-  if (int rc = g.open(file)) return rc;
-  if (!tdio::compare_rasters(a.r, a.path, g.r, g.path)) { printf("File sizes do not match\n%s\n", file); td::set_error("companion grid does not match"); return TD_ERR_MISMATCH; }
-  if (dt == tdio::DT_F32) nodata_msgs(g.r.nodata(), type, (float)g.r.nodata()); else nodata_msgs(g.r.nodata(), type, (int16_t)g.r.nodata());
+  if (int rc = companion_open(a, g, file, dt, type)) return rc;
   return g.read(data, dt);
+}
+
+// TAUDEM_B200_GPUS=N for the five sibling sweep tools (mgpu_sibling): the ranks read their rows of every input, the parent writes
+// the outputs (mapping slot, file, type, nodata) in the order the single-GPU run writes them
+bool use_multi_gpu(const Input& in, int useOutlets) { return td::mgpu_world() > 1 && useOutlets != 1 && in.ny >= td::mgpu_world(); }
+struct SibOut { int slot; const char* file; tdio::DType t; double nodata; };
+int sibling_multi_gpu(td::MgpuSibJob& J, const Input& like, const std::vector<SibOut>& outs, double t0, const char* name) {
+  const int world = td::mgpu_world();
+  const size_t n = (size_t)like.nx * like.ny;
+  size_t bytes[3] = {0, 0, 0};
+  for (const SibOut& o : outs) bytes[o.slot] = n * (o.t == tdio::DT_I16 ? 2 : 4);
+  bool mapped = true;
+  for (int i = 0; i < 3; ++i) if (bytes[i]) { J.out[i] = td::mgpu_alloc_shared(bytes[i]); mapped = mapped && J.out[i]; }
+  auto unmap = [&]() { for (int i = 0; i < 3; ++i) td::mgpu_free_shared(J.out[i], bytes[i]); };
+  if (!mapped) { unmap(); td::set_error("cannot map the shared output rasters"); return TD_ERR_IO; }
+  J.nx = like.nx; J.ny = like.ny;
+  const double t1 = now();
+  double secs = 0.; int rounds = 0;
+  int rc = td::mgpu_sibling(J, world, &secs, &rounds);
+  const double t2 = now();
+  if (rc) printf("%s device error: %s\n", name, td_last_error());
+  for (const SibOut& o : outs) {
+    if (rc) break;
+    rc = o.t == tdio::DT_I16 ? write_like(o.file, like, o.t, o.nodata, (const int16_t*)J.out[o.slot]) : write_like(o.file, like, o.t, o.nodata, (const float*)J.out[o.slot]);
+  }
+  const double t3 = now();
+  unmap();
+  if (rc) return rc;
+  // (the ranks read their rows inside what is reported as compute time: Read time is the header pass)
+  printf("Processors: %d\nRead time: %f\nCompute time: %f\nWrite time: %f\nTotal time: %f\n", world, t1 - t0, t2 - t1, t3 - t2, t3 - t0);
+  printf("Device compute time: %f\nExchange rounds: %d\n", secs, rounds);
+  return TD_OK;
 }
 
 }  // namespace
@@ -504,6 +542,13 @@ int td_d8flowpathextremeup(const char* pfile, const char* safile, const char* ss
   if (useOutlets == 1) { if (int rc = outlet_cells(datasrc, lyrname, uselyrname, lyrno, p, &ocols, &orows)) return rc; }
   std::vector<int16_t> dir;
   nodata_msgs(p.r.nodata(), "int16_t", (int16_t)p.r.nodata());
+  if (use_multi_gpu(p, useOutlets)) {
+    Input a;
+    if (int rc = companion_open(p, a, safile, tdio::DT_F32, "float", "value grid does not match")) return rc;
+    td::MgpuSibJob J;
+    J.tool = td::MgpuSibJob::EXTREMEUP; J.dirfile = pfile; J.in[0] = safile; J.usemax = usemax; J.contcheck = contcheck;
+    return sibling_multi_gpu(J, p, {{0, ssafile, tdio::DT_F32, (double)-3.4028234663852886e38f}}, t0, "D8FlowPathExtremeUp");
+  }
   if (int rc = p.read(&dir, tdio::DT_I16)) return rc;
   Input a; std::vector<float> sa;
   if (int rc = a.open(safile)) return rc;
@@ -540,6 +585,14 @@ int td_gridnet(const char* pfile, const char* plenfile, const char* tlenfile, co
   if (useOutlets == 1) { if (int rc = outlet_cells(datasrc, lyrname, uselyrname, lyrno, p, &ocols, &orows)) return rc; }
   std::vector<int16_t> dir;
   nodata_msgs(p.r.nodata(), "int16_t", (int16_t)p.r.nodata());
+  if (use_multi_gpu(p, useOutlets)) {
+    Input m;
+    if (useMask == 1) { if (int rc = companion_open(p, m, maskfile, tdio::DT_I32, "int32_t", "mask grid does not match")) return rc; }
+    td::MgpuSibJob J;
+    J.tool = td::MgpuSibJob::GRIDNET; J.dirfile = pfile; J.in[0] = useMask == 1 ? maskfile : nullptr; J.thresh = thresh;
+    return sibling_multi_gpu(J, p, {{2, gordfile, tdio::DT_I16, -1.0}, {0, plenfile, tdio::DT_F32, (double)-1.0f}, {1, tlenfile, tdio::DT_F32, (double)-1.0f}},
+                             t0, "GridNet");
+  }
   if (int rc = p.read(&dir, tdio::DT_I16)) return rc;
   Input m; std::vector<int32_t> mask;
   if (useMask == 1) {
@@ -580,6 +633,14 @@ int td_dmarea(const char* angfile, const char* adecfile, const char* dmfile, con
   if (useOutlets == 1) { if (int rc = outlet_cells(datasrc, lyrname, uselyrname, lyrno, a, &ocols, &orows)) return rc; }
   std::vector<float> ang, dm, wg;
   nodata_msgs(a.r.nodata(), "float", (float)a.r.nodata());
+  if (use_multi_gpu(a, useOutlets)) {
+    Input d, w;
+    if (int rc = companion_open(a, d, dmfile, tdio::DT_F32, "float", "decay multiplier grid does not match")) return rc;
+    if (usew) { if (int rc = companion_open(a, w, wfile, tdio::DT_F32, "float", "weight grid does not match")) return rc; }
+    td::MgpuSibJob J;
+    J.tool = td::MgpuSibJob::DECAY; J.dirfile = angfile; J.in[0] = dmfile; J.in[1] = usew ? wfile : nullptr; J.contcheck = contcheck;
+    return sibling_multi_gpu(J, a, {{0, adecfile, tdio::DT_F32, (double)-3.4028234663852886e38f}}, t0, "DinfDecayAccum");
+  }
   if (int rc = a.read(&ang, tdio::DT_F32)) return rc;
   Input d;
   if (int rc = d.open(dmfile)) return rc;
@@ -623,6 +684,15 @@ int td_dsllarea(const char* angfile, const char* ctptfile, const char* dmfile, c
   std::vector<float> ang, dm, q;
   std::vector<int16_t> dg;
   nodata_msgs(a.r.nodata(), "float", (float)a.r.nodata());
+  if (use_multi_gpu(a, useOutlets)) {
+    Input d, g, qq;
+    if (int rc = companion_open(a, d, dmfile, tdio::DT_F32, "float")) return rc;
+    if (int rc = companion_open(a, g, dgfile, tdio::DT_I16, "int16_t")) return rc;
+    if (int rc = companion_open(a, qq, qfile, tdio::DT_F32, "float")) return rc;
+    td::MgpuSibJob J;
+    J.tool = td::MgpuSibJob::CONCLIM; J.dirfile = angfile; J.in[0] = dmfile; J.in[1] = qfile; J.in[2] = dgfile; J.csol = cSol; J.contcheck = contcheck;
+    return sibling_multi_gpu(J, a, {{0, ctptfile, tdio::DT_F32, (double)-3.4028234663852886e38f}}, t0, "DinfConcLimAccum");
+  }
   if (int rc = a.read(&ang, tdio::DT_F32)) return rc;
   Input d, g, qq;
   if (int rc = companion(a, d, dmfile, &dm, tdio::DT_F32, "float")) return rc;
@@ -658,6 +728,17 @@ int td_tlaccum(const char* angfile, const char* tsupfile, const char* tcfile, co
   if (useOutlets == 1) { if (int rc = outlet_cells(datasrc, lyrname, uselyrname, lyrno, a, &ocols, &orows)) return rc; }
   std::vector<float> ang, tsup, tc, cin;
   nodata_msgs(a.r.nodata(), "float", (float)a.r.nodata());
+  if (use_multi_gpu(a, useOutlets)) {
+    Input ts, tcc, ci;
+    if (int rc = companion_open(a, ts, tsupfile, tdio::DT_F32, "float")) return rc;
+    if (int rc = companion_open(a, tcc, tcfile, tdio::DT_F32, "float")) return rc;
+    if (usec == 1) { if (int rc = companion_open(a, ci, cinfile, tdio::DT_F32, "float")) return rc; }
+    td::MgpuSibJob J;
+    J.tool = td::MgpuSibJob::TRANSLIM; J.dirfile = angfile; J.in[0] = tsupfile; J.in[1] = tcfile; J.in[2] = usec == 1 ? cinfile : nullptr; J.contcheck = contcheck;
+    std::vector<SibOut> outs = {{0, tlafile, tdio::DT_F32, (double)-3.4028234663852886e38f}, {1, depfile, tdio::DT_F32, (double)-3.4028234663852886e38f}};
+    if (usec == 1) outs.push_back({2, coutfile, tdio::DT_F32, (double)-3.4028234663852886e38f});
+    return sibling_multi_gpu(J, a, outs, t0, "DinfTransLimAccum");
+  }
   if (int rc = a.read(&ang, tdio::DT_F32)) return rc;
   Input ts, tcc, ci;
   if (int rc = companion(a, ts, tsupfile, &tsup, tdio::DT_F32, "float")) return rc;

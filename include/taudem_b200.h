@@ -199,9 +199,6 @@ void td_ctx_destroy(td_ctx*);
 int td_pitch_for(int nx);        /* smallest legal pitch */
 /* diagnostics: device counter i of the context (27 = tile visits of the last sweep) */
 unsigned long long td_ctx_counter(td_ctx*, int i);
-/* TAUDEM_B200_TIMING=1: milliseconds the last level / walk sweep spent in phase i
- * (0 level passes, 1 ready-list collection, 2 chain walking, 3 rivers); 0 otherwise. */
-unsigned long long td_ctx_sweep_hist(td_ctx*, int i);   /* TAUDEM_B200_TIMING statistics of the last sweep by visit size, see capi.cu */
 
 /* synthetic fractal DEM written straight into a strip (bench/test input generator) */
 int td_gen_dem_dev(float* dem, td_strip s, int row0_global, int total_ny, unsigned seed,

@@ -5,8 +5,7 @@
 With TAUDEM_B200_TIMING=1 the kernel records, per tile visit, the cycles lane 0 spent waiting for a ticket, loading,
 running the wavefront and writing back, the cells evaluated and the wavefront iterations, and counts the visits of carried
 tiles (claimed by the worker that made them ready, without a ticket: their wait is zero).
-TAUDEM_B200_WORKERS=<n> (fewer workers per SM), TAUDEM_B200_POLL=1 (plain nanosleep polling) and TAUDEM_B200_EXP=16 (no carried
-tiles) are experiment knobs of the kernel."""
+TAUDEM_B200_EXP=16 turns the carry off (every activation goes through the ticket queue), for comparison."""
 import os
 import sys
 

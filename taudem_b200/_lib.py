@@ -81,7 +81,6 @@ SIGNATURES = {
     "td_ctx_destroy": (None, [_P]),
     "td_pitch_for": (_I, [_I]),
     "td_ctx_counter": (C.c_ulonglong, [_P, _I]),
-    "td_ctx_sweep_hist": (C.c_ulonglong, [_P, _I]),
     "td_gen_dem_dev": (_I, [_P, Strip, _I, _I, C.c_uint, _F, _F, _P]),
     "td_gen_weights_dev": (_I, [_P, Strip, _I, C.c_uint, _P]),
     "td_flood_init_dev": (_I, [_P, _P, _P, _P, Strip, _F, _I, _P]),

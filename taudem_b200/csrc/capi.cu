@@ -90,16 +90,6 @@ unsigned long long td_ctx_counter(td_ctx* ctx, int i) {
   return v;
 }
 
-// statistics of the last warp sweep (TAUDEM_B200_TIMING): i = 4 * bin + {0 visits, 1 cells, 2 wavefront iterations, 3 wavefront cycles},
-// bins by cells evaluated per visit (< 8, < 32, < 128, more)
-unsigned long long td_ctx_sweep_hist(td_ctx* ctx, int i) {
-  unsigned long long v = 0;
-  if (!ctx || i < 0 || i >= 20 || !ctx->wsched.p) return 0;
-  cudaDeviceSynchronize();
-  cudaMemcpy(&v, ctx->wsched.as<unsigned long long>() + 40 + i, sizeof v, cudaMemcpyDeviceToHost);
-  return v;
-}
-
 
 td_ctx* td_ctx_create(void) {
   if (need_device() != TD_OK) return nullptr;

@@ -44,11 +44,12 @@ struct td_ctx {
   bool peer_G_opened = false;
   Buf peer_halo, gbuf;
   int peer_on = 0;
-  int sweep_dinf = 0;                    // which dependency state node/cnt hold (tile height of the sweep)
+  int sweep_dinf = 0;                    // which dependency state node/cnt hold
   td::PropRow prop;                      // prop() table of the strip whose theta table is loaded (uniform = 0: rows differ)
   double dx0 = 0.;                       // cell size of the strip's rows when they all have the same (prop.uniform)
   double halo_dx[2] = {0., 0.}, halo_dy[2] = {0., 0.};   // cell sizes of the neighbour strips' edge rows (row above / below; <= 0: not set, the strip's own edge rows stand in)
-  int wgrid[16] = {0};           // persistent grid of the four warp-per-tile sweep kernels (D8 / D-infinity x weights) on this context's device
+  static constexpr int SWEEP_KERNELS = 14;   // instantiations of the warp-per-tile sweep kernel (the table SWEEPS in sweep_warp.cu)
+  int wgrid[SWEEP_KERNELS] = {0};         // persistent grid of each of them on this context's device
   unsigned long long* d_ctr = nullptr;   // 32 device counters
   unsigned long long* h_ctr = nullptr;   // pinned host mirror
   td_ctx();

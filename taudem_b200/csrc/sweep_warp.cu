@@ -37,12 +37,11 @@ namespace td {
 namespace {
 
 constexpr int TS = 32;                                // tile width (cells) = lanes of a warp
-// tile height (a multiple of 32: RPL = height / 32 rows per lane).  64-row D8 tiles (13 workers per SM instead of 26) were
-// measured: 330 ms instead of 288 ms at 65536^2 with identical results — the second set of warps hides more latency than the
-// taller tile saves instructions.
-template <bool DINF> constexpr int tile_h() { return 32; }
+constexpr int TH = 32;                                // tile height: one row per lane (64-row D8 tiles were slower: 330 instead of 288 ms at 65536^2)
 constexpr int RS = TS + 4;                            // ring row stride: cell lx of a tile row at lx + 4, its west neighbour at 3, its east neighbour at
                                                       // 36 = slot 0 of the next row (slots 0..2 of a row are otherwise unused): rows stay 16-byte aligned
+constexpr int RH = TH + 2;                            // ring rows
+constexpr int RN = RH * RS + 4;                       // ring array length (the east neighbour of the last ring row lives at RH * RS)
 #ifndef TD_WSTK
 #define TD_WSTK 128
 #endif
@@ -73,21 +72,17 @@ __device__ __forceinline__ int lut_dcol(int k) { return (int)((DCOL_LUT >> (2 * 
 // one worker's shared memory: everything a visit touches while it runs the wavefront
 template <bool DINF>
 struct __align__(16) WarpMem {
-  static constexpr int TH = tile_h<DINF>();      // tile rows
-  static constexpr int RH = TH + 2;              // ring rows
-  static constexpr int RN = RH * RS + 4;         // ring array length (the east neighbour of the last ring row lives at RH * RS)
-  static constexpr int TC = TS * TH;             // cells per tile
   float area[RN];                         // areas of the tile and its ring (-1 = nodata / not final)
   float ang[DINF ? RN : 4];               // D-infinity: angles of the same cells
   unsigned short node[RN];                // node words of the same cells
-  alignas(16) unsigned cnt[TC / 4];       // dependency counts, four cells per word: 0..8 (0 = ready or evaluated by this visit), 0xFE = evaluated
+  alignas(16) unsigned cnt[TS * TH / 4];  // dependency counts, four cells per word: 0..8 (0 = ready or evaluated by this visit), 0xFE = evaluated
                                           // by an earlier visit, 0xFF = not a node
   unsigned short stk[DINF ? STKCAP : 2];  // D-infinity: second receivers that became ready (what does not fit is found again by a rescan of the counts)
-  unsigned short ext[DINF ? 256 : (TH > 32 ? 192 : 128)];   // flow that leaves the tile: source cell | (direction - 1) << 11  (<= 124 / 188 perimeter cells x receivers)
+  unsigned short ext[DINF ? 256 : 128];   // flow that leaves the tile: source cell | (direction - 1) << 11  (<= 124 perimeter cells x receivers)
   unsigned evmask[TH];                    // per tile row: cells evaluated by this visit
   int sp, next, dirty, pad;
 };
-template <bool DINF> constexpr int workers_per_cta() { return DINF ? 16 : (tile_h<false>() > 32 ? 13 : 26); }
+template <bool DINF> constexpr int workers_per_cta() { return DINF ? 16 : 26; }
 static_assert(sizeof(WarpMem<false>) * workers_per_cta<false>() <= 227 * 1024 && sizeof(WarpMem<true>) * workers_per_cta<true>() + 1024 <= 227 * 1024,
               "the workers of a CTA must fit the shared memory of an SM");
 static_assert(offsetof(WarpMem<true>, ang) % 16 == 0 && offsetof(WarpMem<true>, node) % 8 == 0 && offsetof(WarpMem<false>, node) % 8 == 0, "cp.async alignment");
@@ -122,7 +117,7 @@ struct WArgs {
   double dx0;              // the cell size a cell's own area adds (src/areadinf.cpp:216)
   unsigned long long* ctr; // scheduler words (see MAXSH)
   unsigned long long* stat;// [0] carried visits, [1] cells, [2] wavefront iterations, [3] visits, [4..7] cycle statistics (TAUDEM_B200_TIMING)
-  int stats, poll, exp;    // exp: experiment switches (TAUDEM_B200_EXP; EXP_NO_CARRY)
+  int stats, exp;          // exp: TAUDEM_B200_EXP (EXP_NO_CARRY)
   // peer mode (one strip per GPU, the neighbours' buffers mapped over NVLink with CUDA IPC): no exchange rounds — a tile
   // delivers into the neighbour GPU exactly as it delivers into a neighbour tile.  Every GPU only WRITES remote memory
   // (the neighbour's halo-area buffer, counts, tile states, queue); everything it reads is its own.
@@ -152,14 +147,6 @@ __device__ __forceinline__ void cp8(void* smem, const void* g) { cp_check(smem, 
 __device__ __forceinline__ void cp4(void* smem, const void* g) { cp_check(smem, g, 4); memcpy(smem, g, 4); }
 __device__ __forceinline__ void cp_wait_all() {}
 #endif
-
-__device__ __forceinline__ void fence_acq_rel() {
-#ifdef TD_EMU
-  emu::yield();
-#else
-  asm volatile("fence.acq_rel.gpu;" ::: "memory");
-#endif
-}
 
 // ---- scheduler (one lane per worker)
 // In peer mode a neighbour GPU operates on this strip's scheduler words and on the counts of its edge rows with
@@ -249,10 +236,7 @@ __device__ __forceinline__ long long ld_relaxed(const unsigned long long* p) {
 #endif
 }
 // waits about `cycles` SM cycles without touching memory
-__device__ __forceinline__ void idle_wait(unsigned cycles, int plain) {
-#ifndef TD_EMU
-  if (plain) { __nanosleep(cycles >> 1); return; }
-#endif
+__device__ __forceinline__ void idle_wait(unsigned cycles) {
 #ifdef TD_EMU
   (void)cycles; emu::yield();
 #else
@@ -310,7 +294,7 @@ __device__ int sched_pop(const WArgs& a, int q, bool scanner) {
         if (over) { atomicExch(a.ctr + C_TERM, 1ull); return -1; }
       }
     }
-    idle_wait(wait, a.poll);
+    idle_wait(wait);
     if (wait < 4096) wait <<= 1;
   }
 }
@@ -423,11 +407,63 @@ __device__ __forceinline__ float gridnet_eval(const WArgs& a, const Mem& M, int 
   return val;
 }
 
+// The D8 gather (src/aread8.cpp:228-257; ALG 1 / 2: src/D8flowpathextremeup.cpp:182-215; ALG 4-6: gridnet_eval): the value of
+// the cell at ring slot ri (strip row r, column c) from its contributors `msk`; `con` becomes true at a contaminated contributor.
+struct Eval { float val; bool con; };
+template <bool USEW, int ALG, typename Mem>
+__device__ __forceinline__ Eval d8_gather(const WArgs& a, const Mem& M, int ri, unsigned msk, int r, int c, float wv, float NOD, bool con) {
+  if (ALG >= 4) return {gridnet_eval<ALG>(a, M, ri, msk, r, c), con};
+  if (USEW) {
+    float val = (ALG == 0 && nd_f(wv, a.w_nodata)) ? -1.0f : wv;
+#pragma unroll
+    for (int k = 1; k <= 8; ++k)
+      if (msk & (1u << (k - 1))) {
+        const float an = M.area[ri + drow(k) * RS + dcol(k)];
+        if (nd_f(an, NOD)) con = true;
+        else val = ALG == 0 ? val + an : ALG == 1 ? (an > val ? an : val) : (an < val ? an : val);
+      }
+    return {val, con};
+  }
+  // no weights: an area is -1 (nodata: contaminated) or a positive count, and a contaminated contributor contaminates the
+  // cell — its value does not matter then
+  float val = 1.0f, mn = 0.f;
+#pragma unroll
+  for (int k = 1; k <= 8; ++k)
+    if (msk & (1u << (k - 1))) {
+      const float an = M.area[ri + drow(k) * RS + dcol(k)];
+      val = val + an;
+      mn = fminf(mn, an);
+    }
+  if (mn < 0.f) con = true;          // (with -nc no area is ever -1 when it is gathered)
+  return {val, con};
+}
+
+// src/areadinf.cpp:187-218: the share the contributor at ring slot ni (strip row rn) sends along direction kk is prop(its angle, kk).
+// The contributor's node word says how it is obtained (dinf_field): for a regular cell one subtraction from a sector edge and one
+// division by the sector's width (a table constant: div_recip) — the same doubles prop() / dinf_outflow form; irregular cells and
+// strips without a common table take the interval search.
+__device__ __forceinline__ double dinf_share(const WArgs& a, const Sector* sect, unsigned f, float av, int kk, int rn) {
+  if (a.prop.uniform && f != 9u) {
+    const bool upper = f >= 10u;
+    const int k1 = (int)(upper ? f - 8u : f);
+    const bool first = kk == k1 && !upper;
+    const bool wrap = k1 == 8 && !first && !upper;                 // direction 1 from the wrap sector
+    const Sector S = sect[wrap ? 0 : (upper ? k1 - 1 : k1)];
+    double ad = (double)av;
+    if (wrap) ad = (double)(float)(ad - 2.0 * TD_PI);            // prop()'s float-rounded a - 2 PI (src/commonLib.cpp:82)
+    const double num = first ? S.hi - ad : ad - S.lo;
+    return a.prop.safe ? div_recip(num, S.den, S.rden) : num / S.den;
+  }
+  return wshare_full(av, a.prop.uniform ? a.prop.ar[2] : theta_of_row(a.theta, a.s.ny, min(max(rn, 0), a.s.ny + 1)), kk);
+}
+
+// the area a D-infinity cell of strip row r adds itself (src/areadinf.cpp:216): the strip's one cell size, else its row's
+__device__ __forceinline__ double own_area(const WArgs& a, int r) { return a.prop.uniform ? a.dx0 : a.dxc[min(r, a.s.ny) - 1]; }
+
 template <bool DINF, bool USEW, int ALG>
 __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(const WArgs a) {
   extern __shared__ __align__(16) unsigned char dsm[];
   using Mem = WarpMem<DINF>;
-  constexpr int TH = Mem::TH, RH = Mem::RH, RPL = TH / 32;      // tile rows, ring rows, tile rows per lane
   const Strip& s = a.s;
   const int lane = (int)(threadIdx.x & 31u), wid = (int)(threadIdx.x >> 5);
   const unsigned lt = (1u << lane) - 1u;
@@ -454,23 +490,21 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
     const int c0 = tx * TS, r0 = 1 + ty * TH;
 
     // ---- 1. dependency counts: lane = tile row (32 bytes each), before anything else
-    unsigned g0[8 * RPL];
-#pragma unroll
-    for (int rp = 0; rp < RPL; ++rp) {
-      const int row = lane + 32 * rp, r = r0 + row;
+    unsigned g0[8];
+    {
+      const int r = r0 + lane;
       uint4 qa = make_uint4(FULL, FULL, FULL, FULL), qb = qa;
       if (r <= s.ny) {
         const uint4* src = reinterpret_cast<const uint4*>(a.cntw + (s.idx(r, c0) >> 2));
         qa = __ldcg(src); qb = __ldcg(src + 1);
       }
-      unsigned* g = g0 + 8 * rp;
-      g[0] = qa.x; g[1] = qa.y; g[2] = qa.z; g[3] = qa.w; g[4] = qb.x; g[5] = qb.y; g[6] = qb.z; g[7] = qb.w;
-      uint4* dst = reinterpret_cast<uint4*>(M.cnt + row * 8);
+      g0[0] = qa.x; g0[1] = qa.y; g0[2] = qa.z; g0[3] = qa.w; g0[4] = qb.x; g0[5] = qb.y; g0[6] = qb.z; g0[7] = qb.w;
+      uint4* dst = reinterpret_cast<uint4*>(M.cnt + lane * 8);
       dst[0] = qa; dst[1] = qb;
-      M.evmask[row] = 0u;
+      M.evmask[lane] = 0u;
     }
     if (lane == 0) { M.sp = 0; M.next = 0; M.dirty = 0; }
-    if (!(a.exp & 2)) __threadfence();          // the counts first, then the areas they announce (loaded by other lanes: barrier in between)
+    __threadfence();          // the counts first, then the areas they announce (loaded by other lanes: barrier in between)
     __syncwarp();
     // ---- 2. areas, node words (and angles) of the tile and its ring: asynchronous copies straight into shared memory, all in
     //         flight at once (one round trip); what lies below the strip is filled in directly
@@ -514,13 +548,9 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
       M.area[sw] = aw; M.area[se] = ae;
     }
     // ---- 3. cells that are ready (count 0): every lane keeps the ready cells of its own tile row as a bit mask
-    unsigned rdy = 0, rdy2 = 0;             // ready cells of this lane's row(s): rdy = row `lane`, rdy2 = row `lane + 32` (tall tiles)
+    unsigned rdy = 0;
 #pragma unroll
     for (int j = 0; j < 8; ++j) rdy |= zero_nibble(g0[j]) << (4 * j);
-    if (RPL > 1) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) rdy2 |= zero_nibble(g0[(RPL - 1) * 8 + j]) << (4 * j);
-    }
     cp_wait_all();
     __syncwarp();
     if (a.stats && lane == 0) tk2 = clock64();
@@ -531,7 +561,6 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
     int iters = 0;
     for (;;) {
       if (cur < 0 && rdy) { const int b = __ffs(rdy) - 1; rdy &= rdy - 1; cur = lane * TS + b; }
-      if (RPL > 1 && cur < 0 && rdy2) { const int b = __ffs(rdy2) - 1; rdy2 &= rdy2 - 1; cur = (lane + 32) * TS + b; }
       if (DINF) {
         const unsigned idle = __ballot_sync(FULL, cur < 0);
         if (idle) {
@@ -564,75 +593,39 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
           const unsigned msk = nd & 0xffu;
           bool con = (nd & NODE_CON) != 0;
           float val;
-          if (!DINF) {
-            if (ALG >= 4) val = gridnet_eval<ALG>(a, M, ri, msk, r0 + lr, c0 + lx);
-            else if (USEW) {
-              val = (ALG == 0 && nd_f(wv, a.w_nodata)) ? -1.0f : wv;
-#pragma unroll
-              for (int k = 1; k <= 8; ++k)
-                if (msk & (1u << (k - 1))) {
-                  const float an = M.area[ri + drow(k) * RS + dcol(k)];
-                  if (nd_f(an, NOD)) con = true;
-                  else val = ALG == 0 ? val + an : ALG == 1 ? (an > val ? an : val) : (an < val ? an : val);
-                }
-            } else {
-              val = 1.0f;
-              float mn = 0.f;
-#pragma unroll
-              for (int k = 1; k <= 8; ++k)
-                if (msk & (1u << (k - 1))) {
-                  const float an = M.area[ri + drow(k) * RS + dcol(k)];
-                  val = val + an;
-                  mn = fminf(mn, an);
-                }
-              if (mn < 0.f) con = true;
-            }
-          } else {
+          if (!DINF) { const Eval e = d8_gather<USEW, ALG>(a, M, ri, msk, r0 + lr, c0 + lx, wv, NOD, con); val = e.val; con = e.con; }
+          else {
             double prod = 0.;
             if (lane < 8 && ((msk >> lane) & 1u)) {
               const int k = lane + 1;
               const int dr = lut_drow(k);
               const int ni = ri + dr * RS + lut_dcol(k);
-              const int kk = k > 4 ? k - 4 : k + 4;              // the direction from that neighbour to the cell
               const unsigned f = ((unsigned)M.node[ni] >> 8) & 0xfu;
               const float av = M.ang[ni];
               const float an = M.area[ni];
-              double p;
-              if (a.prop.uniform && f != 9u) {
-                const bool upper = f >= 10u;
-                const int k1 = (int)(upper ? f - 8u : f);
-                const bool first = kk == k1 && !upper;
-                const bool wrap = k1 == 8 && !first && !upper;
-                const Sector S = sect[wrap ? 0 : (upper ? k1 - 1 : k1)];
-                double ad = (double)av;
-                if (wrap) ad = (double)(float)(ad - 2.0 * TD_PI);
-                const double num = first ? S.hi - ad : ad - S.lo;
-                p = a.prop.safe ? div_recip(num, S.den, S.rden) : num / S.den;
-              } else {
-                const int rn = r0 + lr + dr;
-                p = wshare_full(av, a.prop.uniform ? a.prop.ar[2] : theta_of_row(a.theta, s.ny, min(max(rn, 0), s.ny + 1)), kk);
-              }
+              const double p = dinf_share(a, sect, f, av, k > 4 ? k - 4 : k + 4, r0 + lr + dr);   // (the direction from that neighbour to the cell)
+              // ALG 3 (src/dinfdecayaccum.cpp:205-235) is written out in each mode: a helper shared with the lane mode costs this
+              // kernel 1-3 registers
               if (ALG == 3) {
                 const float dmv = __ldg(a.dm + s.idx(r0 + lr + dr, c0 + lx + lut_dcol(k)));
                 prod = (nd_f(an, NOD) || nd_f(dmv, a.dm_nodata)) ? __longlong_as_double(0x7ff8dead00000000ll) : (double)(float)((double)(dmv * an) * p);
-              } else
-              prod = nd_f(an, NOD) ? __longlong_as_double(0x7ff8dead00000000ll) : p * (double)an;   // NaN: a contaminated contributor
+              } else prod = nd_f(an, NOD) ? __longlong_as_double(0x7ff8dead00000000ll) : p * (double)an;   // NaN: a contaminated contributor
             }
             val = 0.f;
-            if (ALG == 3) val = USEW ? wv : (float)(a.prop.uniform ? a.dx0 : a.dxc[min(r0 + lr, s.ny) - 1]);
+            if (ALG == 3) val = USEW ? wv : (float)own_area(a, r0 + lr);
             for (unsigned m = msk; m; m &= m - 1u) {               // increasing k: the reference's order of additions
               const double pr = __shfl_sync(FULL, prod, __ffs(m) - 1);
               if (pr != pr) con = true; else val = ALG == 3 ? val + (float)pr : (float)((double)val + pr);
             }
             if (ALG == 3) {}
             else if (USEW) val = val + wv;
-            else val = (float)((double)val + (a.prop.uniform ? a.dx0 : a.dxc[min(r0 + lr, s.ny) - 1]));
+            else val = (float)((double)val + own_area(a, r0 + lr));
           }
           if (con && a.contcheck) val = NOD;
           if (lane == 0) { M.area[ri] = val; M.evmask[lr] |= 1u << lx; }
           int next = -1;
 #pragma unroll
-          for (int j = 0; j < (DINF ? 2 : 1); ++j) {
+          for (int j = 0; j < (DINF ? 2 : 1); ++j) {        // the receivers, classified like the lane mode's below
             int k;
             if (!DINF) k = (int)((nd >> 8) & 0xfu);
             else k = j == 0 ? dinf_node_k1(nd) : dinf_node_k2(nd);
@@ -683,65 +676,21 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
         bool con = (nd & NODE_CON) != 0;
         float val;
         int cont = -1;
-        if (!DINF) {
-          // src/aread8.cpp:228-257
-          if (ALG >= 4) val = gridnet_eval<ALG>(a, M, ri, msk, r0 + lr, c0 + lx);
-          else if (USEW) {
-            val = (ALG == 0 && nd_f(wv, a.w_nodata)) ? -1.0f : wv;
-#pragma unroll
-            for (int k = 1; k <= 8; ++k)
-              if (msk & (1u << (k - 1))) {
-                const float an = M.area[ri + drow(k) * RS + dcol(k)];
-                if (nd_f(an, NOD)) con = true;
-                else val = ALG == 0 ? val + an : ALG == 1 ? (an > val ? an : val) : (an < val ? an : val);
-              }
-          } else {
-            // no weights: an area is -1 (nodata: contaminated) or a positive count, and a contaminated contributor
-            // contaminates the cell — its value does not matter then
-            val = 1.0f;
-            float mn = 0.f;
-#pragma unroll
-            for (int k = 1; k <= 8; ++k)
-              if (msk & (1u << (k - 1))) {
-                const float an = M.area[ri + drow(k) * RS + dcol(k)];
-                val = val + an;
-                mn = fminf(mn, an);
-              }
-            if (mn < 0.f) con = true;          // (with -nc no area is ever -1 when it is gathered)
-          }
-        } else {
-          // src/areadinf.cpp:187-218: the share a contributor sends here is prop(its angle, direction to me).  The
-          // contributor's node word says how it is obtained (dinf_field): for a regular cell one subtraction from a sector
-          // edge and one division by the sector's width (a table constant: div_recip) — the same doubles prop() /
-          // dinf_outflow form; irregular cells and strips without a common table take the interval search.
+        if (!DINF) { const Eval e = d8_gather<USEW, ALG>(a, M, ri, msk, r0 + lr, c0 + lx, wv, NOD, con); val = e.val; con = e.con; }
+        else {
           const int r = r0 + lr;
           val = 0.f;
           float loadin = 0.f;                                    // ALG 9: the load of the second substance that arrives
-          if (ALG == 3) val = USEW ? wv : (float)(a.prop.uniform ? a.dx0 : a.dxc[min(r, s.ny) - 1]);
+          if (ALG == 3) val = USEW ? wv : (float)own_area(a, r);
 #pragma unroll 1
           for (unsigned m = msk; m; m &= m - 1u) {               // increasing k: the reference's order of additions
             const int k = __ffs(m);
             const int dr = lut_drow(k);
             const int ni = ri + dr * RS + lut_dcol(k);
-            const int kk = k > 4 ? k - 4 : k + 4;              // the direction from that neighbour to this cell
             const unsigned f = ((unsigned)M.node[ni] >> 8) & 0xfu;
             const float av = M.ang[ni];
             const float an = M.area[ni];
-            double p;
-            if (a.prop.uniform && f != 9u) {
-              const bool upper = f >= 10u;
-              const int k1 = (int)(upper ? f - 8u : f);
-              const bool first = kk == k1 && !upper;
-              const bool wrap = k1 == 8 && !first && !upper;                 // direction 1 from the wrap sector
-              const Sector S = sect[wrap ? 0 : (upper ? k1 - 1 : k1)];
-              double ad = (double)av;
-              if (wrap) ad = (double)(float)(ad - 2.0 * TD_PI);            // prop()'s float-rounded a - 2 PI (src/commonLib.cpp:82)
-              const double num = first ? S.hi - ad : ad - S.lo;
-              p = a.prop.safe ? div_recip(num, S.den, S.rden) : num / S.den;
-            } else {
-              const int rn = r + dr;
-              p = wshare_full(av, a.prop.uniform ? a.prop.ar[2] : theta_of_row(a.theta, s.ny, min(max(rn, 0), s.ny + 1)), kk);
-            }
+            const double p = dinf_share(a, sect, f, av, k > 4 ? k - 4 : k + 4, r + dr);         // (the direction from that neighbour to this cell)
             if (ALG == 3) {
               const float dmv = __ldg(a.dm + s.idx(r + dr, c0 + lx + lut_dcol(k)));
               if (nd_f(an, NOD) || nd_f(dmv, a.dm_nodata)) con = true;
@@ -801,14 +750,15 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
             }
           }
           else if (USEW) val = val + wv;
-          else val = (float)((double)val + (a.prop.uniform ? a.dx0 : a.dxc[min(r, s.ny) - 1]));
+          else val = (float)((double)val + own_area(a, r));
         }
         if (con && a.contcheck) val = NOD;
         M.area[ri] = val;
         atomicOr(&M.evmask[lr], 1u << lx);
         // (the areas are in shared memory before the counts that announce them are read: every lane that continues with a
         //  receiver does so after the __syncwarp() that ends this iteration)
-        // ---- the receivers: src/aread8.cpp:261-272, src/areadinf.cpp:221-239
+        // ---- the receivers: src/aread8.cpp:261-272, src/areadinf.cpp:221-239.  The one-chain mode above classifies them the same
+        //      way; a helper shared by both modes costs the D-infinity kernels of ALG 3 and 9 a register each.
 #pragma unroll
         for (int j = 0; j < (DINF ? 2 : 1); ++j) {
           int k;
@@ -837,15 +787,11 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
 
     // ---- 5. write back what this visit evaluated (row by row, only rows with evaluated cells), then publish counts and
     //         deliver the crossings
-    unsigned evs[RPL];
-#pragma unroll
-    for (int rp = 0; rp < RPL; ++rp) {
-      evs[rp] = M.evmask[lane + 32 * rp];
-      for (unsigned rows = __ballot_sync(FULL, evs[rp] != 0u); rows; rows &= rows - 1u) {
-        const int lr = __ffs(rows) - 1;
-        const unsigned evr = __shfl_sync(FULL, evs[rp], lr);
-        if ((evr >> lane) & 1u) a.area[s.idx(r0 + lr + 32 * rp, c0 + lane)] = M.area[(lr + 32 * rp + 1) * RS + lane + 4];
-      }
+    const unsigned evs = M.evmask[lane];
+    for (unsigned rows = __ballot_sync(FULL, evs != 0u); rows; rows &= rows - 1u) {
+      const int lr = __ffs(rows) - 1;
+      const unsigned evr = __shfl_sync(FULL, evs, lr);
+      if ((evr >> lane) & 1u) a.area[s.idx(r0 + lr, c0 + lane)] = M.area[(lr + 1) * RS + lane + 4];
     }
     // The counts.  The shared-memory count of a cell this visit evaluated is 0, of any other cell its count at the start
     // minus the arrivals from inside the tile; bytes >= 0x80 (not a node / evaluated before: flow into a cell without a
@@ -854,25 +800,24 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
     // local arrivals.  Words without a cell of the tile's rim (or of the strip's last row, which a neighbour strip feeds)
     // are touched by nobody else while the tile runs: plain stores, before the fence, like the areas.  The others are
     // added atomically after it; a zero byte in the result is a cell that became ready through arrivals from outside meanwhile.
-    unsigned dl[8 * RPL];
-#pragma unroll
-    for (int rp = 0; rp < RPL; ++rp) {
-      const int row = lane + 32 * rp, myr = r0 + row;
-      const bool rimrow = row == 0 || row == TH - 1 || myr >= s.ny;
+    unsigned dl[8];
+    {
+      const int myr = r0 + lane;
+      const bool rimrow = lane == 0 || lane == TH - 1 || myr >= s.ny;
       unsigned* gw = a.cntw + (s.idx(min(myr, s.ny), c0) >> 2);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const unsigned was = g0[8 * rp + j];
-        unsigned now = M.cnt[row * 8 + j];
+        const unsigned was = g0[j];
+        unsigned now = M.cnt[lane * 8 + j];
         const unsigned keep = ((was >> 7) & 0x01010101u) * 0xffu;
         now = (now & ~keep) | (was & keep);
-        const unsigned e4 = (evs[rp] >> (4 * j)) & 0xfu;
-        dl[8 * rp + j] = now - was + ((e4 * 0x00204081u) & 0x01010101u) * 0xfeu;
-        if (j >= 1 && j <= 6 && !rimrow && dl[8 * rp + j] != 0u) { gw[j] = was + dl[8 * rp + j]; dl[8 * rp + j] = 0u; }
+        const unsigned e4 = (evs >> (4 * j)) & 0xfu;
+        dl[j] = now - was + ((e4 * 0x00204081u) & 0x01010101u) * 0xfeu;
+        if (j >= 1 && j <= 6 && !rimrow && dl[j] != 0u) { gw[j] = was + dl[j]; dl[j] = 0u; }
       }
     }
     __syncwarp();
-    if (a.exp & 8) fence_acq_rel(); else __threadfence();          // release by the lanes that publish: every lane's stores (ordered by the barrier) before their atomics
+    __threadfence();          // release by the lanes that publish: every lane's stores (ordered by the barrier) before their atomics
     // flow that leaves the tile first (the neighbours wait for it), then the rim's counts.  Every lane holds back the last tile
     // its crossings made ready (`pend`, crossing `pend_e`); the others it activates at once.
     const int ne = M.next;
@@ -917,17 +862,15 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
       } else if (pend >= 0 && pend != ct) sched_activate(a, pend);   // (the claim or the activation of `ct` covers a lane's own `ct`)
       carry = __shfl_sync(FULL, carry, wl);
     }
-#pragma unroll
-    for (int rp = 0; rp < RPL; ++rp) {
-      const int myr = r0 + lane + 32 * rp;
-      if (myr > s.ny) continue;
+    if (r0 + lane <= s.ny) {
+      const int myr = r0 + lane;
       unsigned* gw = a.cntw + (s.idx(myr, c0) >> 2);
       bool dirty = false;
 #pragma unroll
       for (int j = 0; j < 8; ++j)
-        if (dl[8 * rp + j] != 0u) {
-          const unsigned old = W_ADD_IF(a.peer && (myr == 1 || myr == s.ny), gw + j, dl[8 * rp + j]);
-          if (zero_bytes(old + dl[8 * rp + j])) dirty = true;
+        if (dl[j] != 0u) {
+          const unsigned old = W_ADD_IF(a.peer && (myr == 1 || myr == s.ny), gw + j, dl[j]);
+          if (zero_bytes(old + dl[j])) dirty = true;
         }
       if (dirty) M.dirty = 1;
     }
@@ -937,10 +880,7 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
       sched_finish(a, t, carry < 0);
     }
     if (a.stats) {
-      int ncell = 0;
-#pragma unroll
-      for (int rp = 0; rp < RPL; ++rp) ncell += __popc(evs[rp]);
-      int tot = ncell;
+      int tot = __popc(evs);
 #pragma unroll
       for (int d = 16; d >= 1; d >>= 1) tot += __shfl_xor_sync(FULL, tot, d);
       if (lane == 0) {
@@ -985,9 +925,9 @@ __global__ void k_wsched_reset(unsigned long long* ctr) { for (int i = threadIdx
 int wargs(td_ctx* ctx, WArgs& a, const Strip& s) {
   a.s = s;
   a.area = nullptr; a.w = nullptr; a.ang = nullptr; a.dx0 = 0.; a.usew = 0; a.contcheck = 1; a.w_nodata = 0.f; a.theta = nullptr; a.dxc = nullptr; a.halo = nullptr; a.dm = nullptr; a.dm_nodata = 0.f; a.dist = nullptr;
-  a.th = ctx->sweep_dinf ? tile_h<true>() : tile_h<false>();      // the tile height goes with the dependency state that is loaded
+  a.th = TH;
   a.ntx = (s.nx + TS - 1) / TS; a.nty = (s.ny + a.th - 1) / a.th;
-  a.stats = 0; a.poll = 0; a.exp = 0;
+  a.stats = 0; a.exp = 0;
   a.peer = 0; a.G = nullptr; a.halo_in = nullptr; a.up = PeerStrip(); a.down = PeerStrip();
   const long long nt = (long long)a.ntx * a.nty;
   if (nt > (1ll << 30)) { set_error("strip has too many tiles"); return TD_ERR_ARG; }
@@ -1009,6 +949,37 @@ int wargs(td_ctx* ctx, WArgs& a, const Strip& s) {
   a.cntw = ctx->cnt.as<unsigned>();
   return TD_OK;
 }
+
+// The instantiations of k_sweep_warp: which (D-infinity, weights, algebra) combinations exist and the grids each one requires.
+enum : unsigned { NEED_W = 1, NEED_DM = 2, NEED_DIST = 4, NEED_EXTRA = 8, NEED_DG = 16, NEED_OUT2 = 32, NEED_CIN = 64, NEED_OUT3 = 128 };
+using SweepLaunch = void (*)(const WArgs&, int, int, size_t, cudaStream_t);
+template <bool D, bool U, int A>
+void launch_sweep(const WArgs& a, int g, int threads, size_t smem, cudaStream_t st) {
+  k_sweep_warp<D, U, A><<<g, threads, smem, st>>>(a);
+}
+struct SweepKernel {
+  bool dinf, usew;
+  int alg;
+  unsigned need;           // NEED_* bits
+  const void* kern;        // for the occupancy queries
+  SweepLaunch launch;
+  int threads;
+  size_t smem;
+};
+template <bool D, bool U, int A>
+SweepKernel sweep_kernel(unsigned need) {
+  return {D, U, A, need, (const void*)k_sweep_warp<D, U, A>, launch_sweep<D, U, A>, workers_per_cta<D>() * 32, sizeof(WarpMem<D>) * workers_per_cta<D>()};
+}
+const SweepKernel SWEEPS[] = {
+    sweep_kernel<false, false, 0>(0), sweep_kernel<false, true, 0>(0), sweep_kernel<true, false, 0>(0), sweep_kernel<true, true, 0>(0),
+    sweep_kernel<false, true, 1>(0), sweep_kernel<false, true, 2>(0),
+    sweep_kernel<true, false, 3>(NEED_DM), sweep_kernel<true, true, 3>(NEED_DM),
+    sweep_kernel<false, false, 4>(NEED_DIST), sweep_kernel<false, false, 5>(NEED_DIST), sweep_kernel<false, false, 6>(NEED_DIST),
+    sweep_kernel<true, true, 7>(NEED_W | NEED_DM | NEED_EXTRA | NEED_DG),
+    sweep_kernel<true, true, 8>(NEED_W | NEED_DM | NEED_EXTRA | NEED_OUT2),
+    sweep_kernel<true, true, 9>(NEED_W | NEED_DM | NEED_EXTRA | NEED_OUT2 | NEED_CIN | NEED_OUT3),
+};
+static_assert(sizeof(SWEEPS) / sizeof(SWEEPS[0]) == td_ctx::SWEEP_KERNELS, "td_ctx::wgrid has one slot per sweep kernel");
 }  // namespace
 
 // Queues every tile of the strip (start of a sweep).
@@ -1041,14 +1012,18 @@ int wsweep_apply_halo(td_ctx* ctx, const Strip& s, const int* dec_top, const int
 int wsweep_run(td_ctx* ctx, bool dinf, float* area, const float* w, const float* ang, const Strip& s, float w_nodata, int usew,
                int contcheck, const double* theta, const double* dxc, int* halo, cudaStream_t st, int alg, const float* dm, float dm_nodata,
                const float* dist, const SweepExtra* extra) {
-  if (alg < 0 || alg > 9 || ((alg == 1 || alg == 2) && (dinf || !usew)) || (alg == 3 && (!dinf || !dm)) || (alg >= 4 && alg <= 6 && (dinf || usew || !dist))) {
-    set_error("wsweep_run: the extreme-value algebra is a D8 sweep over a value grid, the decaying accumulation a D-infinity sweep with a multiplier grid");
+  int row = -1;
+  for (int i = 0; i < td_ctx::SWEEP_KERNELS; ++i)
+    if (SWEEPS[i].dinf == dinf && SWEEPS[i].usew == (usew != 0) && SWEEPS[i].alg == alg) row = i;
+  const unsigned have = (w ? NEED_W : 0u) | (dm ? NEED_DM : 0u) | (dist ? NEED_DIST : 0u) |
+                        (extra ? NEED_EXTRA | (extra->dg ? NEED_DG : 0u) | (extra->out2 ? NEED_OUT2 : 0u) | (extra->cin ? NEED_CIN : 0u) | (extra->out3 ? NEED_OUT3 : 0u) : 0u);
+  if (row < 0) { set_error("wsweep_run: no sweep for this algebra with this flow model and weights"); return TD_ERR_ARG; }
+  if (const unsigned miss = SWEEPS[row].need & ~have) {
+    static const char* const grid[8] = {"w", "dm", "dist", "extra", "extra->dg", "extra->out2", "extra->cin", "extra->out3"};
+    set_error(std::string("wsweep_run: algebra ") + std::to_string(alg) + " requires the grid " + grid[__builtin_ctz(miss)]);
     return TD_ERR_ARG;
   }
-  if (alg >= 7 && (!dinf || !usew || !w || !dm || !extra || (alg == 7 && !extra->dg) || (alg >= 8 && !extra->out2) || (alg == 9 && (!extra->cin || !extra->out3)))) {
-    set_error("wsweep_run: the concentration / transport limited accumulations are D-infinity sweeps with all their grids");
-    return TD_ERR_ARG;
-  }
+  const SweepKernel& K = SWEEPS[row];
   if (alg == 9 && ctx->peer_on && ctx->peer_halo.cap < sizeof(float) * 4 * (size_t)s.pitch) {
     set_error("wsweep_run: peer mode of the transport limited accumulation with a concentration needs the halo buffer of sweep_peer_export");
     return TD_ERR_ARG;
@@ -1075,43 +1050,20 @@ int wsweep_run(td_ctx* ctx, bool dinf, float* area, const float* w, const float*
   const char* te = getenv("TAUDEM_B200_TIMING");
   a.stats = (te && atoi(te) > 0) ? 1 : 0;
   if (const char* xe = getenv("TAUDEM_B200_EXP")) a.exp = atoi(xe);
-  const char* pe = getenv("TAUDEM_B200_POLL");
-  a.poll = (pe && atoi(pe) > 0) ? 1 : 0;
   a.dx0 = ctx->dx0;
-  int warps = dinf ? workers_per_cta<true>() : workers_per_cta<false>();
-  if (const char* we = getenv("TAUDEM_B200_WORKERS")) { const int v = atoi(we); if (v >= 1 && v < warps) warps = v; }   // experiments: fewer workers per SM
-  size_t smem = (dinf ? sizeof(WarpMem<true>) : sizeof(WarpMem<false>)) * (size_t)warps;
-  if (const char* pe2 = getenv("TAUDEM_B200_SMEMPAD")) smem = std::max(smem, (size_t)atoi(pe2));                  // experiments: one CTA per SM whatever its size
-  const void* kern = alg == 7 ? (const void*)k_sweep_warp<true, true, 7> : alg == 8 ? (const void*)k_sweep_warp<true, true, 8>
-                   : alg == 9 ? (const void*)k_sweep_warp<true, true, 9> : alg == 4 ? (const void*)k_sweep_warp<false, false, 4> : alg == 5 ? (const void*)k_sweep_warp<false, false, 5>
-                   : alg == 6 ? (const void*)k_sweep_warp<false, false, 6>
-                   : alg == 3 ? (usew ? (const void*)k_sweep_warp<true, true, 3> : (const void*)k_sweep_warp<true, false, 3>)
-                   : dinf ? (usew ? (const void*)k_sweep_warp<true, true, 0> : (const void*)k_sweep_warp<true, false, 0>)
-                          : alg == 1 ? (const void*)k_sweep_warp<false, true, 1> : alg == 2 ? (const void*)k_sweep_warp<false, true, 2>
-                          : (usew ? (const void*)k_sweep_warp<false, true, 0> : (const void*)k_sweep_warp<false, false, 0>);
-  int& per_dev = ctx->wgrid[alg >= 7 ? 6 + alg : alg >= 4 ? 4 + alg : alg == 3 ? 6 + (usew ? 1 : 0) : alg ? 3 + alg : (dinf ? 2 : 0) + (usew ? 1 : 0)];
-  if (!per_dev || getenv("TAUDEM_B200_WORKERS")) {
+  int& per_dev = ctx->wgrid[row];
+  if (!per_dev) {
     int dev = 0, sms = 0, occ = 0;
     TD_CUDA(cudaGetDevice(&dev));
     TD_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    TD_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    TD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, warps * 32, smem));
+    TD_CUDA(cudaFuncSetAttribute(K.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K.smem));
+    TD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, K.kern, K.threads, K.smem));
     if (occ < 1) { set_error("sweep kernel does not fit on an SM"); return TD_ERR_CUDA; }
     per_dev = sms * occ;     // persistent: every CTA is resident, so queue waits cannot deadlock
   }
   const long long nt = (long long)a.ntx * a.nty;
-  const int g = (int)std::min<long long>(per_dev, (nt + warps - 1) / warps);
-  if (alg == 7) k_sweep_warp<true, true, 7><<<g, warps * 32, smem, st>>>(a);
-  else if (alg == 8) k_sweep_warp<true, true, 8><<<g, warps * 32, smem, st>>>(a);
-  else if (alg == 9) k_sweep_warp<true, true, 9><<<g, warps * 32, smem, st>>>(a);
-  else if (alg == 4) k_sweep_warp<false, false, 4><<<g, warps * 32, smem, st>>>(a);
-  else if (alg == 5) k_sweep_warp<false, false, 5><<<g, warps * 32, smem, st>>>(a);
-  else if (alg == 6) k_sweep_warp<false, false, 6><<<g, warps * 32, smem, st>>>(a);
-  else if (alg == 3) { if (usew) k_sweep_warp<true, true, 3><<<g, warps * 32, smem, st>>>(a); else k_sweep_warp<true, false, 3><<<g, warps * 32, smem, st>>>(a); }
-  else if (dinf) { if (usew) k_sweep_warp<true, true, 0><<<g, warps * 32, smem, st>>>(a); else k_sweep_warp<true, false, 0><<<g, warps * 32, smem, st>>>(a); }
-  else if (alg == 1) k_sweep_warp<false, true, 1><<<g, warps * 32, smem, st>>>(a);
-  else if (alg == 2) k_sweep_warp<false, true, 2><<<g, warps * 32, smem, st>>>(a);
-  else { if (usew) k_sweep_warp<false, true, 0><<<g, warps * 32, smem, st>>>(a); else k_sweep_warp<false, false, 0><<<g, warps * 32, smem, st>>>(a); }
+  const int warps = K.threads / 32;
+  K.launch(a, (int)std::min<long long>(per_dev, (nt + warps - 1) / warps), K.threads, K.smem, st);
   TD_LAUNCHED();
   TD_CUDA(cudaGetLastError());
   return TD_OK;

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY — a tiny stand-in for the CUDA runtime and device language so that the
-// queue / count protocols of taudem_b200/csrc/sweep_walk.cu can be executed on a CPU (tests/test_emu.py).
+// queue / count protocols of taudem_b200/csrc/sweep_warp.cu can be executed on a CPU (tests/test_emu.py).
 //
 // Execution model: the blocks of a launch run one after the other; the threads of a block are fibers
 // (ucontext) that a scheduler switches between at every "interesting" point — atomics, acquire loads,

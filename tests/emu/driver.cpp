@@ -265,6 +265,36 @@ extern "C" int emu_sweep(int dinf, int mode, int passes, const void* dir, float*
   return 0;
 }
 
+// One wsweep_run call with the given (dinf, usew, alg) on a 70 x 40 strip whose cells all drain east, with every grid the
+// algebras read present except those whose bit is set in `missing`: 1 w, 2 dm, 4 dist, 8 extra, 16 dg, 32 out2, 64 cin,
+// 128 out3.  Returns wsweep_run's code; an accepted call runs the whole sweep (77: a ready cell was left unevaluated).
+extern "C" int emu_wsweep_call(int dinf, int usew, int alg, unsigned missing) {
+  const int nx = 70, ny = 40;
+  std::vector<short> p((size_t)nx * ny, 1);
+  std::vector<float> ang((size_t)nx * ny, 0.f), wgt((size_t)nx * ny, 1.f);
+  StripState T;
+  build_strip(T, dinf, dinf ? (const void*)ang.data() : (const void*)p.data(), wgt.data(), nx, ny, 0, ny, dinf ? -3.4028234663852886e38f : -32768.f, 30., 30.);
+  td::make_prop_row(T.theta[0], true, &T.ctx.prop); T.ctx.dx0 = 30.; T.ctx.sweep_dinf = dinf ? 1 : 0;
+  const size_t n = (size_t)T.s.cells();
+  std::vector<float> dm(n, 1.f), dist((size_t)ny * 8, 30.f), cin(n, 0.1f), out2(n, 0.f), out3(n, 0.f);
+  std::vector<short> dg(n, 0);
+  td::SweepExtra X;
+  if (!(missing & 16)) X.dg = dg.data();
+  X.csol = 1.f;
+  if (!(missing & 32)) X.out2 = out2.data();
+  if (!(missing & 64)) X.cin = cin.data();
+  if (!(missing & 128)) X.out3 = out3.data();
+  int rc = td::wsweep_begin(&T.ctx, T.s, nullptr);
+  if (!rc)
+    rc = td::wsweep_run(&T.ctx, dinf != 0, T.area.data(), (missing & 1) ? nullptr : T.w.data(), T.ang.data(), T.s, -9999.f, usew, 1, T.theta.data(),
+                        T.dxc.data(), T.halo.data(), nullptr, alg, (missing & 2) ? nullptr : dm.data(), -9999.f, (missing & 4) ? nullptr : dist.data(),
+                        (missing & 8) ? nullptr : &X);
+  if (!rc)
+    for (int r = 1; r <= ny; ++r)
+      for (int c = 0; c < nx; ++c) if (T.cnt[T.s.idx(r, c)] == 0) return 77;
+  return rc;
+}
+
 // the plain-loop dependency state of a single strip (for comparison with the emulated k_deps_* kernels)
 extern "C" int emu_ref_deps(int dinf, const void* dir, unsigned short* node, unsigned char* cnt, int nx, int ny, float dir_nodata, double dx, double dy) {
   StripState S;

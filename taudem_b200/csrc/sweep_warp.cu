@@ -80,7 +80,7 @@ struct __align__(16) WarpMem {
   unsigned short stk[DINF ? STKCAP : 2];  // D-infinity: second receivers that became ready (what does not fit is found again by a rescan of the counts)
   unsigned short ext[DINF ? 256 : 128];   // flow that leaves the tile: source cell | (direction - 1) << 11  (<= 124 perimeter cells x receivers)
   unsigned evmask[TH];                    // per tile row: cells evaluated by this visit
-  int sp, next, dirty, pad;
+  int sp, next, pad[2];
 };
 template <bool DINF> constexpr int workers_per_cta() { return DINF ? 16 : 26; }
 static_assert(sizeof(WarpMem<false>) * workers_per_cta<false>() <= 227 * 1024 && sizeof(WarpMem<true>) * workers_per_cta<true>() + 1024 <= 227 * 1024,
@@ -244,21 +244,48 @@ __device__ __forceinline__ void idle_wait(unsigned cycles) {
   do { __nanosleep(cycles >> 1); } while (clock64() - t0 < (long long)cycles);
 #endif
 }
-// acquire load (orders the loads that follow after it)
-__device__ __forceinline__ long long ld_acquire(const unsigned long long* p) {
+// The visit's two one-sided fences (DESIGN.md §4.1 lists what each one orders).  System scope in peer mode, where a
+// neighbour GPU publishes into this strip's counts with system-scope atomics.  fence.acquire compiles to an L1 invalidate
+// behind the preceding loads, fence.release to a wait for the preceding stores (MEMBAR.ALL); neither is the SC fence of
+// __threadfence().
+__device__ __forceinline__ void fence_acquire(bool sys) {
 #ifdef TD_EMU
-  emu::yield(); return (long long)*((const volatile unsigned long long*)p);
+  (void)sys; emu::yield();
 #else
-  long long v; asm volatile("ld.acquire.gpu.global.s64 %0, [%1];" : "=l"(v) : "l"(p) : "memory"); return v;
+  if (sys) asm volatile("fence.acquire.sys;" ::: "memory");
+  else asm volatile("fence.acquire.gpu;" ::: "memory");
+#endif
+}
+__device__ __forceinline__ void fence_release(bool sys) {
+#ifdef TD_EMU
+  (void)sys; emu::yield();
+#else
+  if (sys) asm volatile("fence.release.sys;" ::: "memory");
+  else asm volatile("fence.release.gpu;" ::: "memory");
+#endif
+}
+// relaxed (strong, past the L1) load of four count words: with fence_acquire after it, an acquire of what they announce
+__device__ __forceinline__ uint4 ld_cnt4(const uint4* p, bool sys) {
+#ifdef TD_EMU
+  (void)sys; return __ldcg(p);
+#else
+  uint4 v;
+  if (sys) asm volatile("ld.relaxed.sys.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
+  else asm volatile("ld.relaxed.gpu.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
+  return v;
 #endif
 }
 // No tile of this strip is queued or running: every push (tail) has been matched by a finished visit (done).  The counters
 // only grow, a tile's own pushes precede its done, and all done counters are read BEFORE all tails: if the sums are equal,
 // they were equal at the moment the last done was read — nothing was running then, so nothing can be pushed any more
-// (except, in peer mode, by a neighbour strip).
+// (except, in peer mode, by a neighbour strip).  The done loads are relaxed and all in flight at once; the one acquire
+// fence behind them keeps every tail load after every done load.
 __device__ bool sched_balanced(const WArgs& a) {
   long long d = 0, t = 0;
-  for (int q = 0; q < a.nsh; ++q) d += ld_acquire(w_done(a.ctr, q));
+#pragma unroll 16
+  for (int q = 0; q < a.nsh; ++q) d += ld_relaxed(w_done(a.ctr, q));
+  fence_acquire(false);
+#pragma unroll 16
   for (int q = 0; q < a.nsh; ++q) t += ld_relaxed(w_tail(a.ctr, q));
   return d == t;
 }
@@ -298,14 +325,21 @@ __device__ int sched_pop(const WArgs& a, int q, bool scanner) {
     if (wait < 4096) wait <<= 1;
   }
 }
-// (every atomic of the visit has returned its result by now — the counts, the deliveries, the activations — and the plain
-//  stores were fenced before them: nothing of the visit is still in flight when the tile is released)
+// The end of a visit of tile t: release it (running -> idle), or queue it again if it was re-activated while it ran or is
+// `dirty` (a rim count of the tile reached zero through arrivals from outside: it has a ready cell).  A dirty tile is still
+// ours (running or running + re-activated: nobody else changes its state then), so it goes straight to queued.
+// (the visit's count atomics — the rim's, the crossings' — have returned their results, consumed for `dirty` and the
+//  activations, before the release is issued, and the plain stores were fenced before them: nothing of the visit that
+//  touches this tile is still in flight when it is released; activations of other tiles may be)
+__device__ __forceinline__ int sched_release(const WArgs& a, int t, bool dirty) {
+  return dirty ? 3 : W_CAS_IF(edge_tile(a, t), a.state + t, 2, 0);
+}
 // A worker that popped a tile owes one `done` for that push.  A tile it carries (claimed at the end of a visit, never pushed)
 // adds nothing to the tails, so a visit that hands over to a carried tile does not pay: the chain of carried visits pays once,
 // when it ends.  Until then the shards stay unbalanced, so nobody can declare the end (nor, in peer mode, the strip passive).
-__device__ void sched_finish(const WArgs& a, int t, bool pay) {
-  const bool sys = edge_tile(a, t);
-  if (W_CAS_IF(sys, a.state + t, 2, 0) != 2) { W_EXCH_IF(sys, a.state + t, 1); sched_push(a, t); }
+// `rel` is what sched_release returned.
+__device__ void sched_finish(const WArgs& a, int t, int rel, bool pay) {
+  if (rel != 2) { W_EXCH_IF(edge_tile(a, t), a.state + t, 1); sched_push(a, t); }
   if (pay) atomicAdd(w_done(a.ctr, t & (a.nsh - 1)), 1ull);
 }
 
@@ -496,15 +530,17 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
       uint4 qa = make_uint4(FULL, FULL, FULL, FULL), qb = qa;
       if (r <= s.ny) {
         const uint4* src = reinterpret_cast<const uint4*>(a.cntw + (s.idx(r, c0) >> 2));
-        qa = __ldcg(src); qb = __ldcg(src + 1);
+        qa = ld_cnt4(src, a.peer); qb = ld_cnt4(src + 1, a.peer);
       }
       g0[0] = qa.x; g0[1] = qa.y; g0[2] = qa.z; g0[3] = qa.w; g0[4] = qb.x; g0[5] = qb.y; g0[6] = qb.z; g0[7] = qb.w;
       uint4* dst = reinterpret_cast<uint4*>(M.cnt + lane * 8);
       dst[0] = qa; dst[1] = qb;
       M.evmask[lane] = 0u;
     }
-    if (lane == 0) { M.sp = 0; M.next = 0; M.dirty = 0; }
-    __threadfence();          // the counts first, then the areas they announce (loaded by other lanes: barrier in between)
+    if (lane == 0) { M.sp = 0; M.next = 0; }
+    // the counts first, then the areas they announce: every lane's acquire covers its own count loads (and lane 0's or
+    // lane wl's claim of the tile); the barrier after it orders them before the other lanes' copies
+    fence_acquire(a.peer);
     __syncwarp();
     // ---- 2. areas, node words (and angles) of the tile and its ring: asynchronous copies straight into shared memory, all in
     //         flight at once (one round trip); what lies below the strip is filled in directly
@@ -817,12 +853,16 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
       }
     }
     __syncwarp();
-    __threadfence();          // release by the lanes that publish: every lane's stores (ordered by the barrier) before their atomics
-    // flow that leaves the tile first (the neighbours wait for it), then the rim's counts.  Every lane holds back the last tile
-    // its crossings made ready (`pend`, crossing `pend_e`); the others it activates at once.
+    fence_release(a.peer);    // every lane's stores (ordered before it by the barrier) before any lane's first atomic
+    // One batch of atomics, all in flight at once: the flow that leaves the tile through each lane's first crossing (e = lane)
+    // and the rim's counts.  Then, from the values they return: the activations (every lane holds back the last tile its
+    // crossings made ready, `pend`, crossing `pend_e`, and activates the others at once), the carry and whether the tile is
+    // dirty.  Crossings beyond the first 32 (a visit that drained much of the tile, not a river's hop) follow one by one.
     const int ne = M.next;
     int pend = -1, pend_e = -1;
-    for (int e = lane; e < ne; e += 32) {
+    // crossing e: its atomic (or halo record / peer delivery); the tile of the target cell, whose count byte (at bit `sh` of
+    // the returned word `old`) it decremented, or -1
+    auto cross = [&](int e, unsigned& old, unsigned& sh) -> int {
       const int l = M.ext[e] & 0x7ff, k = (M.ext[e] >> 11) + 1;
       const int lr = l >> 5, lx = l & 31;
       const int nlr = lr + lut_drow(k), nlx = lx + lut_dcol(k);
@@ -830,55 +870,65 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
       if (r == 0 || r == s.ny + 1) {
         if (a.peer) deliver_peer<ALG>(a, r == 0, c0 + lx, M.area[(lr + 1) * RS + lx + 4], c);   // the source's area is still in shared memory
         else atomicAdd(a.halo + (r == 0 ? 0 : s.pitch) + c, 1);
-        continue;
+        return -1;
       }
-      const unsigned ndr = (unsigned)M.node[(nlr + 1) * RS + nlx + 4];
-      if (!(ndr & NODE_VALID)) continue;
+      if (!((unsigned)M.node[(nlr + 1) * RS + nlx + 4] & NODE_VALID)) return -1;
       const long long ci = s.idx(r, c);
-      const unsigned sh = (unsigned)(ci & 3) * 8u;
-      const unsigned old = W_ADD_IF(a.peer && (r == 1 || r == s.ny), a.cntw + (ci >> 2), 0u - (1u << sh));
-      if (((old >> sh) & 0xffu) == 1u) {
+      sh = (unsigned)(ci & 3) * 8u;
+      old = W_ADD_IF(a.peer && (r == 1 || r == s.ny), a.cntw + (ci >> 2), 0u - (1u << sh));
+      return ((r - 1) / TH) * a.ntx + c / TS;
+    };
+    unsigned xo = 0u, xsh = 0u, ro[8];
+    const int xt = lane < ne ? cross(lane, xo, xsh) : -1;
+    const int myr = r0 + lane;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) ro[j] = 0u;
+    if (myr <= s.ny) {
+      unsigned* gw = a.cntw + (s.idx(myr, c0) >> 2);
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (dl[j] != 0u) ro[j] = W_ADD_IF(a.peer && (myr == 1 || myr == s.ny), gw + j, dl[j]);
+    }
+    if (xt >= 0 && ((xo >> xsh) & 0xffu) == 1u) { pend = xt; pend_e = lane; }
+    for (int e = lane + 32; e < ne; e += 32) {
+      unsigned o, sh;
+      const int tt = cross(e, o, sh);
+      if (tt >= 0 && ((o >> sh) & 0xffu) == 1u) {
         if (pend >= 0) sched_activate(a, pend);
-        pend = ((r - 1) / TH) * a.ntx + c / TS; pend_e = e;
+        pend = tt; pend_e = e;
       }
     }
+    bool dirty = false;
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      if (dl[j] != 0u && zero_bytes(ro[j] + dl[j])) dirty = true;
+    dirty = __ballot_sync(FULL, dirty) != 0u;
     // The carry: of the tiles of this strip made ready by a crossing, the one of the LAST crossing made (normally the river
     // that the one-chain mode followed to the tile's edge) is visited next by this worker, without the ticket queue: claimed
     // idle -> running here, it skips the push, the pop, a waiting worker's back-off and the queue behind other tiles.  A tile
-    // that is queued or running already (or every tile, with EXP_NO_CARRY) is activated as before.
+    // that is queued or running already (or every tile, with EXP_NO_CARRY) is activated as before.  The claim (lane wl) and
+    // the release of this tile (lane 0) go out together.
     int hi = pend_e;
 #pragma unroll
     for (int d = 16; d >= 1; d >>= 1) hi = max(hi, __shfl_xor_sync(FULL, hi, d));
+    const int wl = hi & 31;                                 // crossing e was delivered by lane e % 32
+    const int ct = hi >= 0 ? __shfl_sync(FULL, pend, wl) : -1;
+    int claim = -1, rel = -1;
+    if (hi >= 0 && lane == wl && !(a.exp & EXP_NO_CARRY)) claim = W_CAS_IF(edge_tile(a, ct), a.state + ct, 0, 2);
+    if (lane == 0) rel = sched_release(a, t, dirty);
     if (hi >= 0) {
-      const int wl = hi & 31;                               // crossing e was delivered by lane e % 32
-      const int ct = __shfl_sync(FULL, pend, wl);
       if (lane == wl) {
         // the claim's result is consumed (the branch) before the carried visit loads the tile's counts, so those loads cannot
         // be issued before the claim was performed: whoever delivers into the tile after it re-activates it (2 -> 3)
-        if (!(a.exp & EXP_NO_CARRY) && W_CAS_IF(edge_tile(a, ct), a.state + ct, 0, 2) == 0) {
+        if (claim == 0) {
           carry = ct;
           if (a.stats) atomicAdd(a.stat, 1ull);
         } else sched_activate(a, ct);
       } else if (pend >= 0 && pend != ct) sched_activate(a, pend);   // (the claim or the activation of `ct` covers a lane's own `ct`)
       carry = __shfl_sync(FULL, carry, wl);
     }
-    if (r0 + lane <= s.ny) {
-      const int myr = r0 + lane;
-      unsigned* gw = a.cntw + (s.idx(myr, c0) >> 2);
-      bool dirty = false;
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        if (dl[j] != 0u) {
-          const unsigned old = W_ADD_IF(a.peer && (myr == 1 || myr == s.ny), gw + j, dl[j]);
-          if (zero_bytes(old + dl[j])) dirty = true;
-        }
-      if (dirty) M.dirty = 1;
-    }
-    __syncwarp();
-    if (lane == 0) {
-      if (M.dirty) sched_activate(a, t);
-      sched_finish(a, t, carry < 0);
-    }
+    __syncwarp();             // every lane's pushes before lane 0's done
+    if (lane == 0) sched_finish(a, t, rel, carry < 0);
     if (a.stats) {
       int tot = __popc(evs);
 #pragma unroll

@@ -29,9 +29,9 @@ void set_compute_seconds(double s) { g_compute_s = s; }
 using td::Strip;
 
 td_ctx::td_ctx() {
-  cudaMalloc(&d_ctr, 32 * sizeof(unsigned long long));
-  cudaMallocHost(&h_ctr, 32 * sizeof(unsigned long long));
-  if (d_ctr) cudaMemset(d_ctr, 0, 32 * sizeof(unsigned long long));
+  cudaMalloc(&d_ctr, NCTR * sizeof(unsigned long long));
+  cudaMallocHost(&h_ctr, NCTR * sizeof(unsigned long long));
+  if (d_ctr) cudaMemset(d_ctr, 0, NCTR * sizeof(unsigned long long));
 }
 td_ctx::~td_ctx() {
   node.release(); cnt.release(); lev.release(); mk.release(); listA.release(); listB.release(); listC.release();
@@ -84,7 +84,7 @@ double td_last_compute_seconds(void) { return td::g_compute_s; }
 int td_pitch_for(int nx) { return (nx + 31) / 32 * 32; }
 unsigned long long td_ctx_counter(td_ctx* ctx, int i) {
   unsigned long long v = 0;
-  if (!ctx || i < 0 || i >= 32) return 0;
+  if (!ctx || i < 0 || i >= td_ctx::NCTR) return 0;
   cudaDeviceSynchronize();
   cudaMemcpy(&v, ctx->d_ctr + i, sizeof v, cudaMemcpyDeviceToHost);
   return v;

@@ -50,7 +50,8 @@ struct td_ctx {
   double halo_dx[2] = {0., 0.}, halo_dy[2] = {0., 0.};   // cell sizes of the neighbour strips' edge rows (row above / below; <= 0: not set, the strip's own edge rows stand in)
   static constexpr int SWEEP_KERNELS = 14;   // instantiations of the warp-per-tile sweep kernel (the table SWEEPS in sweep_warp.cu)
   int wgrid[SWEEP_KERNELS] = {0};         // persistent grid of each of them on this context's device
-  unsigned long long* d_ctr = nullptr;   // 32 device counters
+  static constexpr int NCTR = 40;        // device counters: [24..32] the contributing-area sweep's statistics (sweep_warp.cu WArgs::stat)
+  unsigned long long* d_ctr = nullptr;   // NCTR device counters
   unsigned long long* h_ctr = nullptr;   // pinned host mirror
   td_ctx();
   ~td_ctx();

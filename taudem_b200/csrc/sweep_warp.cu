@@ -80,7 +80,7 @@ struct __align__(16) WarpMem {
   unsigned short stk[DINF ? STKCAP : 2];  // D-infinity: second receivers that became ready (what does not fit is found again by a rescan of the counts)
   unsigned short ext[DINF ? 256 : 128];   // flow that leaves the tile: source cell | (direction - 1) << 11  (<= 124 perimeter cells x receivers)
   unsigned evmask[TH];                    // per tile row: cells evaluated by this visit
-  int sp, next, pad[2];
+  int sp, next, ovf, pad;                 // ovf (statistics only): a second receiver did not fit the fork stack in this visit
 };
 template <bool DINF> constexpr int workers_per_cta() { return DINF ? 16 : 26; }
 static_assert(sizeof(WarpMem<false>) * workers_per_cta<false>() <= 227 * 1024 && sizeof(WarpMem<true>) * workers_per_cta<true>() + 1024 <= 227 * 1024,
@@ -116,7 +116,8 @@ struct WArgs {
   PropRow prop;            // D-infinity: the strip's prop() table (prop.uniform: every row has the same cell size dx0) — else per-row angles from `theta`
   double dx0;              // the cell size a cell's own area adds (src/areadinf.cpp:216)
   unsigned long long* ctr; // scheduler words (see MAXSH)
-  unsigned long long* stat;// [0] carried visits, [1] cells, [2] wavefront iterations, [3] visits, [4..7] cycle statistics (TAUDEM_B200_TIMING)
+  unsigned long long* stat;// [0] carried visits, [1] cells, [2] wavefront iterations, [3] visits, [4..7] cycle statistics, [8] visits whose
+                           // fork stack overflowed (more than STKCAP second receivers pending: the rescan of the counts finds the rest) (TAUDEM_B200_TIMING)
   int stats, exp;          // exp: TAUDEM_B200_EXP (EXP_NO_CARRY)
   // peer mode (one strip per GPU, the neighbours' buffers mapped over NVLink with CUDA IPC): no exchange rounds — a tile
   // delivers into the neighbour GPU exactly as it delivers into a neighbour tile.  Every GPU only WRITES remote memory
@@ -384,7 +385,7 @@ __global__ void k_wsched_init(int* state, int* tq, int ntiles, unsigned long lon
   }
   if (i == 0) {
     ctr[C_ACTIVE] = 1ull;
-    for (int j = 0; j < 8; ++j) stat[j] = 0;
+    for (int j = 0; j < 9; ++j) stat[j] = 0;
   }
 }
 
@@ -537,7 +538,7 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
       dst[0] = qa; dst[1] = qb;
       M.evmask[lane] = 0u;
     }
-    if (lane == 0) { M.sp = 0; M.next = 0; }
+    if (lane == 0) { M.sp = 0; M.next = 0; M.ovf = 0; }
     // the counts first, then the areas they announce: every lane's acquire covers its own count loads (and lane 0's or
     // lane wl's claim of the tile); the barrier after it orders them before the other lanes' copies
     fence_acquire(a.peer);
@@ -677,7 +678,7 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
                 if (next < 0) next = l2;
                 else {
                   forked = true;
-                  if (lane == 0) { const int slot = M.sp; if (slot < STKCAP) M.stk[slot] = (unsigned short)l2; M.sp = slot + 1; }
+                  if (lane == 0) { const int slot = M.sp; if (slot < STKCAP) M.stk[slot] = (unsigned short)l2; else if (a.stats) M.ovf = 1; M.sp = slot + 1; }
                 }
               }
             } else if (s.on_grid(r0 + nlr, c0 + nlx)) {
@@ -808,7 +809,10 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
             const unsigned old = atomicSub(&M.cnt[l2 >> 2], 1u << sh);
             if (((old >> sh) & 0xffu) == 1u) {
               if (cont < 0) cont = l2;
-              else { const int slot = atomicAdd(&M.sp, 1); if (slot < STKCAP) M.stk[slot] = (unsigned short)l2; }   // a second ready receiver: an idle lane takes it
+              else {                                                       // a second ready receiver: an idle lane takes it
+                const int slot = atomicAdd(&M.sp, 1);
+                if (slot < STKCAP) M.stk[slot] = (unsigned short)l2; else if (a.stats) M.ovf = 1;
+              }
             }
           } else if (s.on_grid(r0 + nlr, c0 + nlx)) {
             M.ext[atomicAdd(&M.next, 1)] = (unsigned short)(l | ((k - 1) << 11));
@@ -942,6 +946,7 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
         atomicAdd(a.stat + 7, (unsigned long long)(tk4 - tk3));
         atomicAdd(a.stat + 1, (unsigned long long)tot);
         atomicAdd(a.stat + 2, (unsigned long long)iters);
+        if (DINF && M.ovf) atomicAdd(a.stat + 8, 1ull);
       }
     }
     __syncwarp();

@@ -1,5 +1,6 @@
 // TEST INFRASTRUCTURE ONLY — driver.cpp plus one entry point that also hands back the sweep's statistics counters
-// (with TAUDEM_B200_TIMING set: [0] carried visits, [1] cells, [2] wavefront iterations, [3] visits; summed over the strips),
+// (with TAUDEM_B200_TIMING set: [0] carried visits, [1] cells, [2] wavefront iterations, [3] visits, [4..7] cycles, [8] visits whose fork
+// stack overflowed; summed over the strips),
 // which the strips' contexts lose when emu_sweep returns.  tests/test_sweep_carry.py builds it.
 #include "driver.cpp"
 
@@ -40,7 +41,7 @@ extern "C" int emu_sweep_stats(int dinf, const void* dir, float* out, int nx, in
     }
     if (round > 10000) return 2;
   }
-  for (int j = 0; j < 8; ++j) {
+  for (int j = 0; j < 9; ++j) {
     stats[j] = 0;
     for (auto& T : S) stats[j] += T.ctx.d_ctr[24 + j];
   }

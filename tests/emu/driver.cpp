@@ -16,7 +16,7 @@ void set_error(const std::string& m) { g_err = m; }
 int cuda_fail(cudaError_t, const char* what) { g_err = what; return 90; }
 }  // namespace td
 
-td_ctx::td_ctx() { d_ctr = (unsigned long long*)calloc(32, 8); h_ctr = (unsigned long long*)calloc(32, 8); }
+td_ctx::td_ctx() { d_ctr = (unsigned long long*)calloc(NCTR, 8); h_ctr = (unsigned long long*)calloc(NCTR, 8); }
 td_ctx::~td_ctx() {
   free(d_ctr); free(h_ctr);
   node.p = cnt.p = nullptr;       // owned by the caller below

@@ -1,7 +1,8 @@
 """GPU parity: the CUDA path (through the C ABI, host-grid level) against
 (a) the committed golden outputs of the reference's own tools and
 (b) the recorded outputs of the reference tools on larger seeded inputs (tests/golden/reference.json, tests/reference.py)
-Bar: bit-exact fel, p, sd8, slp, ad8; <= 1e-5 relative (identical nodata masks) ang, sca.
+Bar: every raster bit for bit, ang and sca included (DESIGN.md §2).  The 1e-5 relative figure that the project states towards
+its users is not used here: it cannot see a D-infinity contribution lost or counted twice where a river crosses a tile.
 """
 import numpy as np
 import pytest
@@ -11,7 +12,7 @@ import port
 import sibling_cases
 import taudem_b200 as td
 from taudem_b200 import synth
-from util import ANG_ND, FEL_ND, assert_bits, assert_float_parity, golden_cases, load_golden, write_geographic_dem
+from util import ANG_ND, FEL_ND, assert_bits, golden_cases, load_golden, write_geographic_dem
 
 pytestmark = pytest.mark.gpu
 MISSINGFLOAT = np.float32(-3.4028234663852886e38)
@@ -28,13 +29,13 @@ def test_golden(name):
     assert_bits(p, g["p"], "p")
     ang, slp = td.dinfflowdir_grid(g["fel"], dx=dx, dy=dy)
     assert_bits(slp, g["slp"], "slp")
-    assert_float_parity(ang, g["ang"], "ang")
+    assert_bits(ang, g["ang"], "ang")
     assert_bits(td.aread8_grid(g["p"]), g["ad8"], "ad8")
     assert_bits(td.aread8_grid(g["p"], weights=g["w"]), g["ad8_w"], "ad8 -wg")
     assert_bits(td.aread8_grid(g["p"], contcheck=False), g["ad8_nc"], "ad8 -nc")
-    assert_float_parity(td.areadinf_grid(g["ang"], dx=dx, dy=dy), g["sca"], "sca")
-    assert_float_parity(td.areadinf_grid(g["ang"], weights=g["w"], dx=dx, dy=dy), g["sca_w"], "sca -wg")
-    assert_float_parity(td.areadinf_grid(g["ang"], dx=dx, dy=dy, contcheck=False), g["sca_nc"], "sca -nc")
+    assert_bits(td.areadinf_grid(g["ang"], dx=dx, dy=dy), g["sca"], "sca")
+    assert_bits(td.areadinf_grid(g["ang"], weights=g["w"], dx=dx, dy=dy), g["sca_w"], "sca -wg")
+    assert_bits(td.areadinf_grid(g["ang"], dx=dx, dy=dy, contcheck=False), g["sca_nc"], "sca -nc")
 
 
 CASES = [
@@ -57,11 +58,11 @@ def test_recorded_reference(refrun, name, make, dx, dy):
     p, sd8 = td.d8flowdir_grid(fel_r, dx=dx, dy=dy)
     assert_bits(sd8, sd8_r, "sd8"); assert_bits(p, p_r, "p")
     ang, slp = td.dinfflowdir_grid(fel_r, dx=dx, dy=dy)
-    assert_bits(slp, slp_r, "slp"); assert_float_parity(ang, ang_r, "ang")
+    assert_bits(slp, slp_r, "slp"); assert_bits(ang, ang_r, "ang")
     assert_bits(td.aread8_grid(p_r), R.aread8(p_r), "ad8")
     assert_bits(td.aread8_grid(p_r, weights=w, contcheck=False), R.aread8(p_r, weights=w, contcheck=False), "ad8 -wg -nc")
-    assert_float_parity(td.areadinf_grid(ang_r, dx=dx, dy=dy), R.areadinf(ang_r), "sca")
-    assert_float_parity(td.areadinf_grid(ang_r, weights=w, dx=dx, dy=dy), R.areadinf(ang_r, weights=w), "sca -wg")
+    assert_bits(td.areadinf_grid(ang_r, dx=dx, dy=dy), R.areadinf(ang_r), "sca")
+    assert_bits(td.areadinf_grid(ang_r, weights=w, dx=dx, dy=dy), R.areadinf(ang_r, weights=w), "sca -wg")
     # ... and end to end: D8 chain is bit-exact from the raw DEM
     p2, _ = td.d8flowdir_grid(td.pitremove_grid(dem), dx=dx, dy=dy)
     assert_bits(td.aread8_grid(p2), R.aread8(p_r), "ad8 end-to-end")
@@ -95,8 +96,8 @@ def test_file_level_cli(refrun, tmp_path):
     assert_bits(td.read_raster(str(d / "demsd8.tif")), sd8_r, "sd8 file")
     assert_bits(td.read_raster(str(d / "demad8.tif")), ad8_r, "ad8 file")
     assert_bits(td.read_raster(str(d / "demslp.tif")), slp_r, "slp file")
-    assert_float_parity(td.read_raster(str(d / "demang.tif")), ang_r, "ang file")
-    assert_float_parity(td.read_raster(str(d / "demsca.tif")), sca_r, "sca file")
+    assert_bits(td.read_raster(str(d / "demang.tif")), ang_r, "ang file")
+    assert_bits(td.read_raster(str(d / "demsca.tif")), sca_r, "sca file")
     # nodata tags round-trip like the reference's (SURVEY.md 8(b) file contract)
     for f, nd in (("demfel.tif", -3.0e38), ("demp.tif", -32768), ("demad8.tif", -1.0), ("demang.tif", ANG_ND)):
         assert np.float32(td.raster_info(str(d / f))["nodata"]) == np.float32(nd)
@@ -216,15 +217,15 @@ def crossings():
 
 def test_sweep_with_many_tile_crossings_matches_the_reference(refrun, crossings):
     """2100 x 3000 cells (6 200 tiles of the dataflow sweep, rivers that cross hundreds of tiles, thousands of tile
-    re-activations): ad8 bit for bit, sca within the tolerance, with and without weights, against the reference tools."""
+    re-activations): ad8 and sca bit for bit, with and without weights, against the reference tools."""
     fel, p, _, ang = crossings
     w = synth.gen_weights(*p.shape)
     R = refrun.RefPipeline(np_ranks=8)
     ad8 = td.aread8_grid(p)
     assert_bits(ad8, R.aread8(p), "ad8")
     assert_bits(td.aread8_grid(p, weights=w, contcheck=False), R.aread8(p, weights=w, contcheck=False), "ad8 -wg -nc")
-    assert_float_parity(td.areadinf_grid(ang), R.areadinf(ang), "sca")
-    assert_float_parity(td.areadinf_grid(ang, weights=w, contcheck=False), R.areadinf(ang, weights=w, contcheck=False), "sca -wg -nc")
+    assert_bits(td.areadinf_grid(ang), R.areadinf(ang), "sca")
+    assert_bits(td.areadinf_grid(ang, weights=w, contcheck=False), R.areadinf(ang, weights=w, contcheck=False), "sca -wg -nc")
     assert ad8.max() > 1e5
 
 
@@ -269,9 +270,9 @@ def test_edge_shapes_against_c_restatement():
         assert_bits(p, p_o, f"p {dem.shape}"); assert_bits(sd8, sd8_o, f"sd8 {dem.shape}")
         ang, slp = td.dinfflowdir_grid(fel, dx=10.0, dy=12.0)
         ang_o, slp_o = port.dinfflowdir(fel, dx=10.0, dy=12.0)
-        assert_bits(slp, slp_o, f"slp {dem.shape}"); assert_float_parity(ang, ang_o, f"ang {dem.shape}")
+        assert_bits(slp, slp_o, f"slp {dem.shape}"); assert_bits(ang, ang_o, f"ang {dem.shape}")
         assert_bits(td.aread8_grid(p_o, weights=w), port.aread8(p_o, weights=w), f"ad8 {dem.shape}")
-        assert_float_parity(td.areadinf_grid(ang_o, dx=10.0, dy=12.0), port.areadinf(ang_o, dx=10.0, dy=12.0), f"sca {dem.shape}")
+        assert_bits(td.areadinf_grid(ang_o, dx=10.0, dy=12.0), port.areadinf(ang_o, dx=10.0, dy=12.0), f"sca {dem.shape}")
 
 
 def test_odd_direction_codes_and_nodata_weights():
@@ -300,8 +301,8 @@ def test_large_vs_c_restatement():
     assert_bits(p, p_o, "p"); assert_bits(sd8, sd8_o, "sd8")
     assert_bits(td.aread8_grid(p), port.aread8(p_o), "ad8")
     ang, slp = td.dinfflowdir_grid(fel); ang_o, slp_o = port.dinfflowdir(fel)
-    assert_bits(slp, slp_o, "slp"); assert_float_parity(ang, ang_o, "ang")
-    assert_float_parity(td.areadinf_grid(ang_o), port.areadinf(ang_o), "sca")
+    assert_bits(slp, slp_o, "slp"); assert_bits(ang, ang_o, "ang")
+    assert_bits(td.areadinf_grid(ang_o), port.areadinf(ang_o), "sca")
 
 
 def test_depression_mask():
@@ -348,9 +349,9 @@ def test_geographic_dem_file_level(refrun, tmp_path):
     assert td.setdir(q("fel.tif"), q("ang.tif"), q("slp.tif")) == 0
     assert td.aread8(q("p.tif"), q("ad8.tif")) == 0
     assert td.area(q("ang.tif"), q("sca.tif")) == 0
-    for n, dt, exact in (("fel", np.float32, True), ("p", np.int16, True), ("sd8", np.float32, True), ("slp", np.float32, True),
-                         ("ad8", np.float32, True), ("ang", np.float32, False), ("sca", np.float32, False)):
-        (assert_bits if exact else assert_float_parity)(td.read_raster(q(n + ".tif"), dt), x[n], n + " (geographic)")
+    for n, dt in (("fel", np.float32), ("p", np.int16), ("sd8", np.float32), ("slp", np.float32), ("ad8", np.float32), ("ang", np.float32),
+                  ("sca", np.float32)):
+        assert_bits(td.read_raster(q(n + ".tif"), dt), x[n], n + " (geographic)")
     assert td.raster_info(q("sca.tif"))["is_geographic"]        # GeoTIFF keys pass through to the outputs
     # the same on row strips (TAUDEM_B200_GPUS=N behind the executables): rows of different cell sizes on both sides of a strip
     # boundary — the halo row of a strip is evaluated with the neighbour row's cell sizes like the reference does (getdxdyc(jn))
@@ -832,7 +833,7 @@ def _bfs_grid_threads():
 @pytest.mark.parametrize("name", list(flat_cases.CASES))
 def test_flat_cases_against_the_reference(refrun, tmp_path, name):
     """Each flat case (tests/flat_cases.py) through d8flowdir_grid / dinfflowdir_grid against the reference (its stored outputs,
-    recomputed by the restatement), square cells and dx != dy: p, sd8, slp bit for bit, ang within the bar.  port.flat_stats()
+    recomputed by the restatement), square cells and dx != dy: p, sd8, slp and ang bit for bit.  port.flat_stats()
     of every reference call shows that the case reaches what it claims; for the pockets, a BFS level larger than one pass of the
     fixed BFS grid on this device."""
     dem, fel = flat_cases.CASES[name]()
@@ -852,7 +853,7 @@ def test_flat_cases_against_the_reference(refrun, tmp_path, name):
             assert_bits(sd8, ref[1], f"sd8 {what}"); assert_bits(p, ref[0], f"p {what}")
         else:
             ang, slp = td.dinfflowdir_grid(fel, dx=dx, dy=dy)
-            assert_bits(slp, ref[1], f"slp {what}"); assert_float_parity(ang, ref[0], f"ang {what}")
+            assert_bits(slp, ref[1], f"slp {what}"); assert_bits(ang, ref[0], f"ang {what}")
 
 
 @pytest.mark.parametrize("name", ["deep_lake", "pockets"])
@@ -902,7 +903,7 @@ def test_flat_resolution_on_row_strips(name, tmp_path):
     p_o, sd8_o = port.d8flowdir(fel, dx=dx, dy=dy)
     assert_bits(td.read_raster(str(d / "p_1.tif"), np.int16), p_o, "p"); assert_bits(td.read_raster(str(d / "sd8_1.tif")), sd8_o, "sd8")
     ang_o, slp_o = port.dinfflowdir(fel, dx=dx, dy=dy)
-    assert_float_parity(td.read_raster(str(d / "ang_1.tif")), ang_o, "ang"); assert_bits(td.read_raster(str(d / "slp_1.tif")), slp_o, "slp")
+    assert_bits(td.read_raster(str(d / "ang_1.tif")), ang_o, "ang"); assert_bits(td.read_raster(str(d / "slp_1.tif")), slp_o, "slp")
 
 
 def test_flat_needing_32767_passes_is_an_error(tmp_path):

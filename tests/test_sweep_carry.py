@@ -19,8 +19,8 @@ MISS = -3.4028234663852886e38
 TS = 32                       # tile edge of the sweep
 
 
-@pytest.fixture(scope="module")
-def emu():
+def build_lib():
+    """the emulation library with emu_sweep_stats (tests/emu/carry_driver.cpp)"""
     test_emu._build()                                  # the transformed kernel sources and the test library
     so = os.path.join(test_emu.BUILD, "libemu_carry.so")
     srcs = [os.path.join(test_emu.EMU, f) for f in ("carry_driver.cpp", "emu.cpp")]
@@ -35,16 +35,21 @@ def emu():
     return lib
 
 
+@pytest.fixture(scope="module")
+def emu():
+    return build_lib()
+
+
 def _sweep(lib, dinf, d, contcheck, seed, nstrips=1):
-    """(result raster, [carried visits, cells, wavefront iterations, visits]) of one emulated sweep"""
+    """(result raster, [carried visits, cells, wavefront iterations, visits, fork-stack overflows]) of one emulated sweep"""
     ny, nx = d.shape
     d = np.ascontiguousarray(d)
     out = np.empty((ny, nx), np.float32)
-    st = np.zeros(8, np.uint64)
+    st = np.zeros(9, np.uint64)
     rc = lib.emu_sweep_stats(int(dinf), d.ctypes.data, out.ctypes.data, nx, ny, MISS if dinf else -32768.0, int(contcheck), 30.0, 30.0,
                              seed, nstrips, st.ctypes.data)
     assert rc == 0
-    return out, [int(v) for v in st[:4]]
+    return out, [int(v) for v in st[:4]] + [int(st[8])]
 
 
 def _channel(ny=192, nx=320, pitch=6):
@@ -111,7 +116,7 @@ def test_channel_matches_the_oracle_and_is_carried(emu, channel, monkeypatch):
     ad8_nc = port.aread8(p, contcheck=False)
     assert ad8_nc.max() > 9000
     for dinf, d, ref, what in ((False, p, ad8_nc, "ad8 -nc"), (True, ang, port.areadinf(ang, contcheck=False), "sca -nc")):
-        out, (carried, cells, _, visits) = _sweep(emu, dinf, d, False, 3 + dinf)
+        out, (carried, cells, _, visits, _) = _sweep(emu, dinf, d, False, 3 + dinf)
         assert_bits(out, ref, what)
         assert cells == p.size
         assert carried >= entries - 10, f"{what}: {carried} carried visits, the river enters a tile {entries} times"

@@ -32,19 +32,32 @@ def assert_bits(a, b, what):
         assert digest(a) == digest(b), f"{what}: differs from the reference's output ({a!r} vs {b!r})"
         return
     if not bits_equal(a, b):
-        bad = np.argwhere(a != b) if a.shape == b.shape else []
-        raise AssertionError(f"{what}: {len(bad)} of {a.size} cells differ; first {[(tuple(i), a[tuple(i)], b[tuple(i)]) for i in bad[:5]]}")
+        raise AssertionError(f"{what}: {bits_report(a, b)}")
 
 
-def assert_float_parity(a, b, what, rtol=1e-5):
-    """The north-star tolerance for D-infinity angle / sca floats: identical nodata/flat masks
-    (values <= -1) and 1e-5 relative elsewhere."""
-    ma, mb = a <= -1, b <= -1
-    assert np.array_equal(ma, mb), f"{what}: nodata masks differ in {(ma != mb).sum()} cells"
-    ok = ~ma
-    rel = np.abs(a[ok].astype(np.float64) - b[ok]) / np.maximum(np.abs(b[ok].astype(np.float64)), 1e-300)
-    assert rel.size == 0 or rel.max() <= rtol, f"{what}: max rel err {rel.max()}"
-    assert bits_equal(a[ma], b[ma]), f"{what}: nodata values differ"
+def ulp_distance(a, b):
+    """per cell: how many float32 values lie between a and b (0 where the bits are equal; +0 and -0 are 1 apart)"""
+    def ordered(x):
+        i = np.ascontiguousarray(x, np.float32).view(np.int32).astype(np.int64)
+        return np.where(i < 0, -(i & 0x7fffffff) - 1, i)
+    return np.abs(ordered(a) - ordered(b))
+
+
+def bits_report(a, b, first=5):
+    """what differs between two rasters: the number of differing cells, for floats the largest ulp distance, and the first
+    cells as (row, column, got, want)"""
+    a, b = np.asarray(a), np.asarray(b)
+    if a.dtype != b.dtype or a.shape != b.shape:
+        return f"{a.dtype}{a.shape} vs {b.dtype}{b.shape}"
+    if a.dtype == np.float32:
+        diff = a.view(np.uint32) != b.view(np.uint32)
+    else:
+        diff = a != b
+    bad = np.argwhere(diff)
+    msg = f"{len(bad)} of {a.size} cells differ"
+    if a.dtype == np.float32 and len(bad):
+        msg += f", by up to {int(ulp_distance(a[diff], b[diff]).max())} ulp"
+    return msg + f"; first {[(*map(int, i), a[tuple(i)].item(), b[tuple(i)].item()) for i in bad[:first]]}"
 
 
 def write_geographic_dem(path, dem, lon0=-111.8, lat0=41.9, cell=0.001, nodata=-9999.0):

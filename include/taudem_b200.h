@@ -159,6 +159,16 @@ int td_slopearea(const char* slopefile, const char* scafile, const char* safile,
 int td_atanbgrid(const char* slopefile, const char* areafile, const char* atanbfile);
 int td_slopearea_host(const float* slp, const float* sca, float* sa, int nx, int ny, float m, float n);
 int td_slopearearatio_host(const float* slp, const float* sca, float* sar, int nx, int ny, float sca_nodata);
+/* The two stream definitions besides the area threshold.  File level = `int peukerdouglas(char* felfile, char* ssfile, float* p)`
+ * (src/PeukerDouglas.cpp:54; p = the smoothing weights of the centre, side and diagonal cells, default 0.4 0.1 0.05) and
+ * `int lengtharea(char* plenfile, char* ad8file, char* ssfile, float* p)` (src/LengthArea.cpp:51; p[0] = M, p[1] = y: ss = 1 where
+ * ad8 >= M plen^y, ad8 read as 32-bit integers; TD_ERR_ARG when the two grids do not match; the output takes ad8's georeference).
+ * peukerdouglas ss: int16, 0 / 1 on every cell, nodata tag -2; lengtharea ss: int16, nodata -32768 where plen < 0.
+ * Both bit-exact (lengtharea's power: see pointwise.cu). */
+int td_peukerdouglas(const char* felfile, const char* ssfile, const float* p /* w_mid, w_side, w_diag */);
+int td_lengtharea(const char* plenfile, const char* ad8file, const char* ssfile, const float* p /* M, y */);
+int td_peukerdouglas_host(const float* fel, int16_t* ss, int nx, int ny, float fel_nodata, const float* p);
+int td_lengtharea_host(const float* plen, const int32_t* ad8, int16_t* ss, int nx, int ny, float m, float y);
 
 /* aread8 + areadinf of one DEM in one call (no weights, no outlets), the host<->device copies overlapped with the kernels
  * on three streams: p in -> aread8 || ang in -> areadinf || ad8 out -> sca out.  Same results as the two calls above.
@@ -348,6 +358,12 @@ int td_threshold_dev(td_ctx*, const float* ssa, const float* mask, int16_t* src,
 int td_twi_dev(td_ctx*, const float* slp, const float* sca, float* twi, td_strip s, float slp_nodata, float sca_nodata, void* stream);
 int td_slopearea_dev(td_ctx*, const float* slp, const float* sca, float* sa, td_strip s, float m, float n, void* stream);
 int td_slopearearatio_dev(td_ctx*, const float* slp, const float* sca, float* sar, td_strip s, float sca_nodata, void* stream);
+/* peukerdouglas on row strips: td_peukerdouglas_smooth_dev (fel with valid halo rows -> the smoothed grid sm; p: host array of the
+ * three weights), then the caller copies the first / last owned rows of sm into the neighbours' halo rows (the reference's second
+ * share()), then td_peukerdouglas_mark_dev (sm -> ss).  fel_nodata: the elevations' nodata value, in both passes.               */
+int td_peukerdouglas_smooth_dev(td_ctx*, const float* fel, float* sm, td_strip s, float fel_nodata, const float* p, void* stream);
+int td_peukerdouglas_mark_dev(td_ctx*, const float* sm, int16_t* ss, td_strip s, float fel_nodata, void* stream);
+int td_lengtharea_dev(td_ctx*, const float* plen, const int32_t* ad8, int16_t* ss, td_strip s, float m, float y, void* stream);
 
 /* Peer mode (one process per GPU on one NVSwitch box): every rank exports the IPC handles of the buffers
  * its neighbours write (counts, tile scheduler, halo areas, rank 0 also the global pending counter), opens

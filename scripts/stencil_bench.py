@@ -38,7 +38,8 @@ def main():
         ts = sorted(ts[1:])                      # the first launch pays module load / tensor map / occupancy query
         best, med = ts[0], ts[len(ts) // 2]
         out[name] = {"ms_best": round(best, 3), "ms_median": round(med, 3), "alg_B_per_cell": bytes_per_cell,
-                     "GB_per_s": round(bytes_per_cell * mc / med, 1), "frac_of_hbm_peak": round(bytes_per_cell * mc / med / peak, 3)}
+                     "GB_per_s": round(bytes_per_cell * mc / med, 1), "frac_of_hbm_peak": round(bytes_per_cell * mc / med / peak, 3),
+                     "frac_of_3350_gbs": round(bytes_per_cell * mc / med / 3350.0, 3)}
         print(f"{name:18s} best {best:8.3f} ms  median {med:8.3f} ms  {bytes_per_cell:2d} B/cell  {bytes_per_cell * mc / med:7.1f} GB/s  {100 * bytes_per_cell * mc / med / peak:5.1f} % of {peak:.0f} GB/s")
 
     dem = T.gen_dem(s, hurst=0.8, tilt=1.0)
@@ -58,7 +59,7 @@ def main():
     sca = s.empty(torch.float32)
     run("k_deps_dinf", 4, lambda: T.areadinf_deps(s, ang, sca, dxc, dyc))
     run("k_deps_dinf (+7 scratch)", 11, lambda: T.areadinf_deps(s, ang, sca, dxc, dyc))
-    if only is not None and not (only & {"k_threshold", "k_twi", "k_slopearea", "k_slopearearatio"}):
+    if only is not None and not (only & {"k_threshold", "k_twi", "k_slopearea", "k_slopearearatio", "k_pd_smooth", "k_pd_mark", "k_lengtharea"}):
         print(json.dumps({"n": n, "hbm_peak_gbs": peak, "kernels": out}))
         return
     # point-wise consumers on the rasters of the path
@@ -68,6 +69,14 @@ def main():
     run("k_twi", 12, lambda: T.l.td_twi_dev(T.ctx, _p(slp), _p(sca), _p(o), s.c, C.c_float(-1.0), C.c_float(-1.0), T._stream()))
     run("k_slopearea", 12, lambda: T.l.td_slopearea_dev(T.ctx, _p(slp), _p(sca), _p(o), s.c, C.c_float(2.0), C.c_float(1.0), T._stream()))
     run("k_slopearearatio", 12, lambda: T.l.td_slopearearatio_dev(T.ctx, _p(slp), _p(sca), _p(o), s.c, C.c_float(-1.0), T._stream()))
+    # the stream definitions: Peuker-Douglas's two passes on fel, length-area on a path length (the D8 area stands in) and ad8 as int32
+    sm = s.empty(torch.float32); ss = s.empty(torch.int16)
+    wts = torch.tensor([0.4, 0.1, 0.05], dtype=torch.float32)
+    B = lambda *ts: sum(t.element_size() for t in ts)      # noqa: E731  (bytes per cell from the rasters read and written)
+    run("k_pd_smooth", B(fel, sm), lambda: T.l.td_peukerdouglas_smooth_dev(T.ctx, _p(fel), _p(sm), s.c, C.c_float(-3.0e38), wts.data_ptr(), T._stream()))
+    run("k_pd_mark", B(sm, ss), lambda: T.l.td_peukerdouglas_mark_dev(T.ctx, _p(sm), _p(ss), s.c, C.c_float(-3.0e38), T._stream()))
+    ad8i = ad8.round().to(torch.int32)
+    run("k_lengtharea", B(ad8, ad8i, ss), lambda: T.l.td_lengtharea_dev(T.ctx, _p(ad8), _p(ad8i), _p(ss), s.c, C.c_float(0.03), C.c_float(1.3), T._stream()))
     print(json.dumps({"n": n, "hbm_peak_gbs": peak, "kernels": out}))
 
 

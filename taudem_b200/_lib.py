@@ -61,6 +61,13 @@ SIGNATURES = {
     "td_slopearearatio_dev": (_I, [_P, _P, _P, _P, Strip, _F, _P]),
     "td_threshold_dev": (_I, [_P, _P, _P, _P, Strip, _F, _F, _P]),
     "td_twi_dev": (_I, [_P, _P, _P, _P, Strip, _F, _F, _P]),
+    "td_peukerdouglas": (_I, [_S, _S, _P]),
+    "td_lengtharea": (_I, [_S, _S, _S, _P]),
+    "td_peukerdouglas_host": (_I, [_P, _P, _I, _I, _F, _P]),
+    "td_lengtharea_host": (_I, [_P, _P, _P, _I, _I, _F, _F]),
+    "td_peukerdouglas_smooth_dev": (_I, [_P, _P, _P, Strip, _F, _P, _P]),
+    "td_peukerdouglas_mark_dev": (_I, [_P, _P, _P, Strip, _F, _P]),
+    "td_lengtharea_dev": (_I, [_P, _P, _P, _P, Strip, _F, _F, _P]),
     "td_nameadd": (_I, [_S, _S, _S]),
     "td_raster_info": (_I, [_S] + [_P] * 9),
     "td_raster_read": (_I, [_S, _I, _P, _I, _I]),

@@ -273,6 +273,37 @@ def slopearearatio_grid(slp, sca, sca_nodata=-1.0):
     return sar
 
 
+def peukerdouglas_grid(fel, weights=(0.4, 0.1, 0.05), nodata=-3.0e38):
+    """Peuker-Douglas stream sources (td_peukerdouglas_host; src/PeukerDouglas.cpp:109-212): the elevations smoothed with the centre,
+    side and diagonal weights, then 1 on every cell that is not the highest of any group of four cells around it (and not on the
+    grid's edge, not nodata, not next to nodata), else 0.  int16, 0 / 1 everywhere (the file's nodata tag is -2)."""
+    fel = _grid(fel, np.float32)
+    ny, nx = fel.shape
+    w = np.ascontiguousarray(weights, np.float32)
+    if w.shape != (3,):
+        raise ValueError("peukerdouglas_grid: three weights (middle, side, diagonal)")
+    ss = np.empty((ny, nx), np.int16)
+    check(lib().td_peukerdouglas_host(_ptr(fel), _ptr(ss), nx, ny, np.float32(nodata), _ptr(w)))
+    return ss
+
+
+def lengtharea_grid(plen, ad8, m=0.03, y=1.3):
+    """Length-area stream sources (td_lengtharea_host; src/LengthArea.cpp:110-120): 1 where ad8 >= m * plen^y, else 0, and -32768
+    where plen < 0.  ad8 must be int32 (the reference reads the contributing area as 32-bit integers, rounding half away from zero:
+    read_raster(path, np.int32) does the same)."""
+    plen = _grid(plen, np.float32)
+    a = np.asarray(ad8)
+    if a.dtype != np.int32:
+        raise TypeError(f"lengtharea_grid: ad8 must be int32, not {a.dtype}")
+    a = np.ascontiguousarray(a)
+    ny, nx = plen.shape
+    if a.shape != plen.shape:
+        raise ValueError("lengtharea_grid: plen and ad8 differ in shape")
+    ss = np.empty((ny, nx), np.int16)
+    check(lib().td_lengtharea_host(_ptr(plen), _ptr(a), _ptr(ss), nx, ny, np.float32(m), np.float32(y)))
+    return ss
+
+
 def contributing_areas_grid(p, ang, p_nodata=int(MISSINGSHORT), ang_nodata=float(MISSINGFLOAT), dx=30.0, dy=30.0, contcheck=True, out_ad8=None, out_sca=None):
     """aread8 + areadinf of one DEM in one call, copies overlapped with the kernels (td_contributing_areas_host)."""
     p = _grid(p, np.int16); ang = _grid(ang, np.float32)

@@ -825,6 +825,58 @@ int td_twi_host(const float* slp, const float* sca, float* twi, int nx, int ny, 
   return TD_OK;
 }
 
+// ---- the stream definitions of Peuker-Douglas (peuker.cu) and length-area (pointwise.cu)
+int td_peukerdouglas_smooth_dev(td_ctx*, const float* fel, float* sm, td_strip s, float fel_nodata, const float* p, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  if (!fel || !sm || !p) { td::set_error("td_peukerdouglas_smooth_dev: bad arguments"); return TD_ERR_ARG; }
+  return td::launch_pd_smooth(fel, sm, Strip(s), fel_nodata, p, (cudaStream_t)stream);
+}
+int td_peukerdouglas_mark_dev(td_ctx*, const float* sm, int16_t* ss, td_strip s, float fel_nodata, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  if (!sm || !ss) { td::set_error("td_peukerdouglas_mark_dev: bad arguments"); return TD_ERR_ARG; }
+  return td::launch_pd_mark(sm, ss, Strip(s), fel_nodata, (cudaStream_t)stream);
+}
+int td_lengtharea_dev(td_ctx*, const float* plen, const int32_t* ad8, int16_t* ss, td_strip s, float m, float y, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  if (!plen || !ad8 || !ss) { td::set_error("td_lengtharea_dev: bad arguments"); return TD_ERR_ARG; }
+  return td::launch_lengtharea(plen, ad8, ss, Strip(s), m, y, (cudaStream_t)stream);
+}
+int td_peukerdouglas_host(const float* fel, int16_t* ss, int nx, int ny, float fel_nodata, const float* p) {
+  if (int rc = need_device()) return rc;
+  if (!fel || !ss || !p || nx <= 0 || ny <= 0) { td::set_error("td_peukerdouglas_host: bad arguments"); return TD_ERR_ARG; }
+  td_ctx* ctx = default_ctx();
+  const td_strip s = host_strip(nx, ny);
+  const size_t n = (size_t)Strip(s).cells();
+  cudaStream_t st = 0;
+  TD_CUDA(ctx->io[0].ensure(n * 4)); TD_CUDA(ctx->io[1].ensure(n * 4)); TD_CUDA(ctx->io[2].ensure(n * 2));
+  float* d_fel = ctx->io[0].as<float>(); float* d_s = ctx->io[1].as<float>(); int16_t* d_ss = ctx->io[2].as<int16_t>();
+  TD_CUDA(h2d(d_fel, fel, s, st));
+  Timer t; t.start(st);
+  if (int rc = td_peukerdouglas_smooth_dev(ctx, d_fel, d_s, s, fel_nodata, p, st)) return rc;
+  if (int rc = td_peukerdouglas_mark_dev(ctx, d_s, d_ss, s, fel_nodata, st)) return rc;
+  td::set_compute_seconds(t.stop(st));
+  TD_CUDA(d2h(ss, d_ss, s, st));
+  TD_CUDA(cudaStreamSynchronize(st));
+  return TD_OK;
+}
+int td_lengtharea_host(const float* plen, const int32_t* ad8, int16_t* ss, int nx, int ny, float m, float y) {
+  if (int rc = need_device()) return rc;
+  if (!plen || !ad8 || !ss || nx <= 0 || ny <= 0) { td::set_error("td_lengtharea_host: bad arguments"); return TD_ERR_ARG; }
+  td_ctx* ctx = default_ctx();
+  const td_strip s = host_strip(nx, ny);
+  const size_t n = (size_t)Strip(s).cells();
+  cudaStream_t st = 0;
+  TD_CUDA(ctx->io[0].ensure(n * 4)); TD_CUDA(ctx->io[1].ensure(n * 4)); TD_CUDA(ctx->io[2].ensure(n * 2));
+  float* d_plen = ctx->io[0].as<float>(); int32_t* d_ad8 = ctx->io[1].as<int32_t>(); int16_t* d_ss = ctx->io[2].as<int16_t>();
+  TD_CUDA(h2d(d_plen, plen, s, st)); TD_CUDA(h2d(d_ad8, ad8, s, st));
+  Timer t; t.start(st);
+  if (int rc = td_lengtharea_dev(ctx, d_plen, d_ad8, d_ss, s, m, y, st)) return rc;
+  td::set_compute_seconds(t.stop(st));
+  TD_CUDA(d2h(ss, d_ss, s, st));
+  TD_CUDA(cudaStreamSynchronize(st));
+  return TD_OK;
+}
+
 // aread8 + areadinf of one DEM in ONE call with the copies overlapped with the kernels: three streams — host -> device (p, then
 // ang), compute (aread8 as soon as p has arrived, areadinf as soon as ang has and aread8 is done), device -> host (ad8 while
 // areadinf runs, then sca).  Same kernels, same results as td_aread8_host followed by td_area_host (no weights, no outlets).

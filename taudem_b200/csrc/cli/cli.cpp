@@ -1,4 +1,5 @@
-// Command line front ends: pitremove, d8flowdir, dinfflowdir, aread8, areadinf (+ the point-wise consumers threshold, twi, slopearea, slopearearatio).
+// Command line front ends: pitremove, d8flowdir, dinfflowdir, aread8, areadinf (+ the point-wise consumers threshold, twi, slopearea, slopearearatio,
+// the sibling sweep tools and the stream definitions peukerdouglas and lengtharea).
 // Same flags, same two invocation styles and the same "print usage and exit(0)" error
 // behaviour as the reference mains (src/PitRemovemn.cpp:48-172, src/D8FlowDirmn.cpp:49-146,
 // src/DinfFlowDirmn.cpp:54-147, src/aread8mn.cpp:49-193, src/areadinfmn.cpp:49-178);
@@ -17,7 +18,7 @@ static int done() { fflush(stdout); fflush(stderr); _exit(0); return 0; }
 
 struct Opt {
   const char* flag;
-  int kind;        // 0 = file name, 1 = switch, 2 = integer, 3 = float (ival points to a float), 4 = two floats
+  int kind;        // 0 = file name, 1 = switch, 2 = integer, 3 = float (ival points to a float), 4 = two floats, 5 = three floats
   char* sval;      // kind 0
   int* ival;       // kind 1 (set to `set`) / kind 2 (parsed) / kind 0 (set to `set` when given, may be NULL)
   int set;
@@ -44,6 +45,7 @@ static void parse(int argc, char** argv, Opt* opts, int nopts) {
     if (o->kind == 0) { strncpy(o->sval, argv[i], MAXLN - 1); o->sval[MAXLN - 1] = 0; if (o->ival) *o->ival = o->set; }
     else if (o->kind == 3) sscanf(argv[i], "%f", (float*)o->ival);
     else if (o->kind == 4) { if (argc <= i + 1) usage(argv[0]); sscanf(argv[i], "%f", (float*)o->ival); i++; sscanf(argv[i], "%f", (float*)o->ival + 1); }
+    else if (o->kind == 5) { if (argc <= i + 2) usage(argv[0]); for (int k = 0; k < 3; ++k, ++i) sscanf(argv[i], "%f", (float*)o->ival + k); i--; }
     else sscanf(argv[i], "%d", o->ival);
     i++;
   }
@@ -431,6 +433,60 @@ int main(int argc, char** argv) {
   if (argc == 2) { td_nameadd(sca, argv[1], "sca"); td_nameadd(slp, argv[1], "slp"); td_nameadd(sar, argv[1], "sar"); }
   int err = td_atanbgrid(slp, sca, sar);
   if (err != 0) printf("Slope area ratio error %d\n", err);
+  return done();
+}
+
+#elif defined(TOOL_peukerdouglas)
+// src/PeukerDouglasmn.cpp:53-128 (no "Error:" preamble; -par takes three floats)
+static void usage(const char* prog) {
+  printf("Simple Use:\n %s <basefilename>\n", prog);
+  printf("Use with specific file names:\n %s -fel <elevationfile>\n", prog);
+  printf("-ss <streamsource> [-par <weightMiddle> <weightSide> <weightDiagonal>]\n");
+  printf("<basefilename> is the name of the base digital elevation model without suffixes for simple input. 'fel' will be appended. \n");
+  printf("<elevationfile> is the name of the elevation input file.\n");
+  printf("<streamsource> is the name of the stream source file output.\n");
+  printf("The elevation input is smoothed by averaging using the center and eight surrounding grid cells.\n");
+  printf("<weightMiddle> is the weight given to the center cell in the smoothing of the input elevations.\n");
+  printf("<weightSide> is the weight given to the 4 side cells in the smoothing of the input elevations.\n");
+  printf("<weightDiagonal> is the weight given to the 4 diagonal cells in the smoothing of the input elevations.\n");
+  printf("Default weights are 0.4 0.1 0.05 if -par is not specified.\n");
+  exit(0);
+}
+int main(int argc, char** argv) {
+  static char fel[MAXLN], ss[MAXLN];
+  float par[3] = {0.4f, 0.1f, 0.05f};
+  if (argc < 2) usage(argv[0]);
+  Opt opts[] = {{"-fel", 0, fel, NULL, 0}, {"-ss", 0, ss, NULL, 0}, {"-par", 5, NULL, (int*)par, 0}};
+  parse(argc, argv, opts, 3);
+  if (argc == 2) { td_nameadd(fel, argv[1], "fel"); td_nameadd(ss, argv[1], "ss"); }
+  int err = td_peukerdouglas(fel, ss, par);
+  if (err != 0) printf("Peuker Douglas Error %d\n", err);
+  return done();
+}
+
+#elif defined(TOOL_lengtharea)
+// src/LengthAreamn.cpp:50-133 (no "Error:" preamble; -par takes two floats)
+static void usage(const char* prog) {
+  printf("Simple Use:\n %s <basefilename>\n", prog);
+  printf("Use with specific file names:\n %s -plen <plenfile>\n", prog);
+  printf("-ad8 <ad8file> -ss <ssfile> [-par <M> <y>] \n");
+  printf("<basefilename> is the name of the base digital elevation model without suffixes for simple input. Suffixes 'plen', 'ad8' and 'ss' will be appended. \n");
+  printf("<plenfile> is the name of the input upslope longest path length file.\n");
+  printf("<ad8file> is the name of input contributing area file.\n");
+  printf("<ssfile> is the name of the output file with the result A >= M L^y ? 1:0.\n");
+  printf("<M> is the coefficient, default value 0.03 if not specified.\n");
+  printf("<y> is the exponent on upslope length, default value 1.3 if not specified.\n");
+  exit(0);
+}
+int main(int argc, char** argv) {
+  static char plen[MAXLN], ad8[MAXLN], ss[MAXLN];
+  float par[2] = {0.03f, 1.3f};
+  if (argc < 2) usage(argv[0]);
+  Opt opts[] = {{"-plen", 0, plen, NULL, 0}, {"-ad8", 0, ad8, NULL, 0}, {"-ss", 0, ss, NULL, 0}, {"-par", 4, NULL, (int*)par, 0}};
+  parse(argc, argv, opts, 4);
+  if (argc == 2) { td_nameadd(plen, argv[1], "plen"); td_nameadd(ad8, argv[1], "ad8"); td_nameadd(ss, argv[1], "ss"); }
+  int err = td_lengtharea(plen, ad8, ss, par);
+  if (err != 0) printf("Length Area Error %d\n", err);
   return done();
 }
 #else

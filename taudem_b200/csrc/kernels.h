@@ -46,6 +46,9 @@ int launch_threshold(const float* ssa, const float* mask, short* src, const Stri
 int launch_slopearea(const float* slp, const float* sca, float* sa, const Strip& s, float m, float n, cudaStream_t st);
 int launch_slopearearatio(const float* slp, const float* sca, float* sar, const Strip& s, float sca_nodata, cudaStream_t st);
 int launch_twi(const float* slp, const float* sca, float* twi, const Strip& s, float slp_nodata, float sca_nodata, cudaStream_t st);
+int launch_lengtharea(const float* plen, const int* ad8, short* ss, const Strip& s, float m, float y, cudaStream_t st);
+int launch_pd_smooth(const float* fel, float* sm, const Strip& s, float nodata, const float* p /* host: w_mid, w_side, w_diag */, cudaStream_t st);
+int launch_pd_mark(const float* sm, short* ss, const Strip& s, float nodata, cudaStream_t st);
 int launch_mask_ok(const int* mask, float* ok, const Strip& s, int thresh, cudaStream_t st);
 int launch_gord_finish(const float* g, const short* p, const float* ok, const unsigned short* node, short* gord, const Strip& s, short p_nodata,
                        int outlets, cudaStream_t st);

@@ -12,12 +12,13 @@ struct MgpuJob {
   float* out = nullptr;         // nx * ny floats in a mapping from mgpu_alloc_shared: every rank stores its rows
 };
 // the other three tools of the path on row strips: tool 0 = pitremove (out0 = fel), 1 = d8flowdir (out0 = p int16, out1 = sd8),
-// 2 = dinfflowdir (out0 = ang, out1 = slp); the rasters live in mappings from mgpu_alloc_shared
+// 2 = dinfflowdir (out0 = ang, out1 = slp), 3 = peukerdouglas (out0 = ss int16); the rasters live in mappings from mgpu_alloc_shared
 struct MgpuFlowJob {
   int tool = 0;
   const char* demfile = nullptr;
   const char* maskfile = nullptr;   // pitremove: depression mask (use_mask)
   int use_mask = 0, four = 0;
+  float par[3] = {0.4f, 0.1f, 0.05f};   // peukerdouglas: smoothing weights
   int nx = 0, ny = 0;
   void* out0 = nullptr;
   float* out1 = nullptr;

@@ -3,6 +3,7 @@
 //   twi        twi = ln(sca / slp) where both are data and positive, else nodata (-1)     (src/TWI.cpp:108-124)
 //   slopearea  sa = slp^m * sca^n where slp >= 0 and sca >= 0, else nodata (-1)            (src/SlopeArea.cpp:114-125)
 //   slopearearatio  sar = slp / sca where sca is data, else nodata (-1)                    (src/SlopeAreaRatio.cpp:107-118)
+//   lengtharea ss = ad8 >= M plen^y ? 1 : 0 where plen >= 0, else nodata (-32768)          (src/LengthArea.cpp:110-120)
 // One streaming kernel each, four cells per thread (16-byte loads, 8 / 16-byte stores): 6 B (10 with a mask) and 12 B of HBM
 // traffic per cell.  Device-strip level entry points take strips like every other kernel of the path; the host-grid level
 // copies dense arrays in and out.  isNodata is linearpart's |v - nodata| < 1e-5 (src/linearpart.h:471-483).
@@ -69,6 +70,24 @@ __global__ void __launch_bounds__(256) k_slopearea(const float* __restrict__ slp
     out[i] = ok ? pow_float(sl[i], m) * pow_float(ar[i], n) : -1.0f;
   }
   *reinterpret_cast<float4*>(sa + o) = make_float4(out[0], out[1], out[2], out[3]);
+}
+// lengtharea (src/LengthArea.cpp:110-120): ss = ((float)ad8 >= M * plen^y) ? 1 : 0 where plen >= 0, else nodata (-32768); ad8 is
+// the contributing area read as 32-bit integers, plen^y as above and M * plen^y one float product.  The reference's powf is within
+// 0.52 ulp, pow_float correctly rounded in all but ~1e-9 of the cases: the power can differ by one ulp, and the result only when
+// (float)ad8 lies exactly on one of those two adjacent floats (tests: bit for bit).  10 B of HBM traffic per cell.
+__global__ void __launch_bounds__(256) k_lengtharea(const float* __restrict__ plen, const int* __restrict__ ad8, short* __restrict__ ss, Strip s,
+                                                    float m, float y) {
+  const int r = 1 + (int)blockIdx.x, c = ((int)blockIdx.y * 256 + (int)threadIdx.x) * 4;
+  if (c >= s.pitch) return;
+  const long long o = s.idx(r, c);
+  const float4 lv = *reinterpret_cast<const float4*>(plen + o);
+  const int4 av = *reinterpret_cast<const int4*>(ad8 + o);
+  const float l[4] = {lv.x, lv.y, lv.z, lv.w};
+  const int a[4] = {av.x, av.y, av.z, av.w};
+  short out[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) out[i] = l[i] >= 0.0f ? (short)((float)a[i] >= m * pow_float(l[i], y) ? 1 : 0) : TD_MISSINGSHORT;
+  *reinterpret_cast<short4*>(ss + o) = make_short4(out[0], out[1], out[2], out[3]);
 }
 // slp / sca as one IEEE float division (-prec-div=true); only the area's nodata is looked at, like the reference
 __global__ void __launch_bounds__(256) k_slopearearatio(const float* __restrict__ slp, const float* __restrict__ sca, float* __restrict__ sar, Strip s,
@@ -148,6 +167,13 @@ int launch_threshold(const float* ssa, const float* mask, short* src, const Stri
 int launch_slopearea(const float* slp, const float* sca, float* sa, const Strip& s, float m, float n, cudaStream_t st) {
   const dim3 grid((unsigned)s.ny, (unsigned)(((s.pitch >> 2) + 255) / 256));
   k_slopearea<<<grid, 256, 0, st>>>(slp, sca, sa, s, m, n);
+  TD_LAUNCHED();
+  TD_CUDA(cudaGetLastError());
+  return TD_OK;
+}
+int launch_lengtharea(const float* plen, const int* ad8, short* ss, const Strip& s, float m, float y, cudaStream_t st) {
+  const dim3 grid((unsigned)s.ny, (unsigned)(((s.pitch >> 2) + 255) / 256));
+  k_lengtharea<<<grid, 256, 0, st>>>(plen, ad8, ss, s, m, y);
   TD_LAUNCHED();
   TD_CUDA(cudaGetLastError());
   return TD_OK;

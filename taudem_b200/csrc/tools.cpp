@@ -114,23 +114,26 @@ int area_multi_gpu(int dinf, int world, const Input& in, const char* infile, con
   return TD_OK;
 }
 
-// the same for pitremove / d8flowdir / dinfflowdir (mgpu_flow): the ranks read their rows of the DEM, the parent writes the rasters
+// the same for pitremove / d8flowdir / dinfflowdir / peukerdouglas (mgpu_flow): the ranks read their rows of the DEM, the parent
+// writes the rasters
 int flow_multi_gpu(int tool, int world, const Input& dem, const char* demfile, const char* maskfile, int use_mask, int four, const char* out0file,
-                   const char* out1file, double t0, double t1) {
+                   const char* out1file, double t0, double t1, const float* par = nullptr) {
   const size_t n = (size_t)dem.nx * dem.ny;
-  const size_t b0 = n * (tool == 1 ? 2 : 4), b1 = tool == 0 ? 0 : n * 4;
+  const size_t b0 = n * (tool == 1 || tool == 3 ? 2 : 4), b1 = (tool == 0 || tool == 3) ? 0 : n * 4;
   void* out0 = td::mgpu_alloc_shared(b0);
   float* out1 = b1 ? (float*)td::mgpu_alloc_shared(b1) : nullptr;
   if (!out0 || (b1 && !out1)) { td::mgpu_free_shared(out0, b0); td::mgpu_free_shared(out1, b1); td::set_error("cannot map the shared output rasters"); return TD_ERR_IO; }
   td::MgpuFlowJob J;
   J.tool = tool; J.demfile = demfile; J.maskfile = maskfile; J.use_mask = use_mask; J.four = four; J.nx = dem.nx; J.ny = dem.ny; J.out0 = out0; J.out1 = out1;
+  if (par) for (int i = 0; i < 3; ++i) J.par[i] = par[i];
   double secs = 0.; int rounds = 0; long long left = 0;
   int rc = td::mgpu_flow(J, world, &secs, &rounds, &left);
   const double t2 = now();
-  const char* name = tool == 0 ? "PitRemove" : tool == 1 ? "D8FlowDir" : "DinfFlowDir";
+  const char* name = tool == 0 ? "PitRemove" : tool == 1 ? "D8FlowDir" : tool == 2 ? "DinfFlowDir" : "PeukerDouglas";
   double t3 = t2, t4 = t2;
   if (rc) printf("%s device error: %s\n", name, td_last_error());
   else if (tool == 0) { rc = write_like(out0file, dem, tdio::DT_F32, (double)-3.0e38f, (const float*)out0); t3 = t4 = now(); }
+  else if (tool == 3) { rc = write_like(out0file, dem, tdio::DT_I16, (double)(int16_t)-2, (const int16_t*)out0); t3 = t4 = now(); }
   else {
     rc = write_like(out1file, dem, tdio::DT_F32, (double)-1.0f, (const float*)out1);            // slope first, like the reference
     t3 = now();
@@ -143,10 +146,13 @@ int flow_multi_gpu(int tool, int world, const Input& dem, const char* demfile, c
   // (the ranks read their rows inside what is reported as compute time; the header pass is the read time)
   if (tool == 0)
     printf("Processes: %d\nHeader read time: %f\nData read time: %f\nCompute time: %f\nWrite time: %f\nTotal time: %f\n", world, t1 - t0, 0.0, t2 - t1, t3 - t2, t3 - t0);
+  else if (tool == 3)
+    printf("Processors: %d\nRead time: %f\nCompute time: %f\nWrite time: %f\nTotal time: %f\n", world, t1 - t0, t2 - t1, t3 - t2, t3 - t0);
   else
     printf("Processors: %d\nHeader read time: %f\nData read time: %f\nCompute Slope time: %f\nWrite Slope time: %f\nResolve Flat time: %f\nWrite Flat time: %f\nTotal time: %f\n",
            world, t1 - t0, 0.0, t2 - t1, t3 - t2, 0.0, t4 - t3, t4 - t0);
-  printf("Device compute time: %f\nExchange rounds: %d\nFlat cells left: %lld\n", secs, rounds, left);
+  if (tool == 3) printf("Device compute time: %f\nExchange rounds: %d\n", secs, rounds);
+  else printf("Device compute time: %f\nExchange rounds: %d\nFlat cells left: %lld\n", secs, rounds, left);
   return TD_OK;
 }
 
@@ -865,6 +871,70 @@ int td_slopearea(const char* slopefile, const char* scafile, const char* safile,
 }
 int td_atanbgrid(const char* slopefile, const char* areafile, const char* atanbfile) try {
   return two_in_one_out(1, "SlopeAreaRatio", slopefile, areafile, atanbfile, nullptr);
+} catch (const std::exception& e) {
+  td::set_error(std::string("exception: ") + e.what());
+  return TD_ERR_IO;
+}
+
+// src/PeukerDouglas.cpp:54-241: fel in, ss out (int16, nodata tag -2, georeference of fel); TAUDEM_B200_GPUS=N runs it on N row strips
+int td_peukerdouglas(const char* felfile, const char* ssfile, const float* p) try {
+  if (!p) { td::set_error("td_peukerdouglas: the weights are missing"); return TD_ERR_ARG; }
+  printf("PeukerDouglas version %s\n", td_version());
+  fflush(stdout);
+  const double t0 = now();
+  Input fel;
+  if (int rc = fel.open(felfile)) return rc;
+  nodata_msgs(fel.r.nodata(), "float", (float)fel.r.nodata());
+  if (td::mgpu_world() > 1 && fel.ny >= td::mgpu_world())
+    return flow_multi_gpu(3, td::mgpu_world(), fel, felfile, nullptr, 0, 0, ssfile, nullptr, t0, now(), p);
+  Warmup warm;
+  std::vector<float> z;
+  if (int rc = fel.read(&z, tdio::DT_F32)) return rc;
+  warm.join();
+  const double t1 = now();
+  std::vector<int16_t> ss((size_t)fel.nx * fel.ny);
+  if (int rc = td_peukerdouglas_host(z.data(), ss.data(), fel.nx, fel.ny, (float)fel.r.nodata(), p)) {
+    printf("PeukerDouglas device error: %s\n", td_last_error());
+    return rc;
+  }
+  const double t2 = now();
+  if (int rc = write_like(ssfile, fel, tdio::DT_I16, (double)(int16_t)-2, ss)) return rc;
+  const double t3 = now();
+  printf("Processors: 1\nRead time: %f\nCompute time: %f\nWrite time: %f\nTotal time: %f\n", t1 - t0, t2 - t1, t3 - t2, t3 - t0);
+  printf("Device compute time: %f\n", td_last_compute_seconds());
+  return TD_OK;
+} catch (const std::exception& e) {
+  td::set_error(std::string("exception: ") + e.what());
+  return TD_ERR_IO;
+}
+
+// src/LengthArea.cpp:51-149: plen (float) and ad8 (read as int32) in, ss out (int16, nodata -32768, georeference of ad8)
+int td_lengtharea(const char* plenfile, const char* ad8file, const char* ssfile, const float* p) try {
+  if (!p) { td::set_error("td_lengtharea: the coefficient and exponent are missing"); return TD_ERR_ARG; }
+  printf("LengthArea version %s\n", td_version());
+  const double t0 = now();
+  Input pl;
+  if (int rc = pl.open(plenfile)) return rc;
+  std::vector<float> plen;
+  nodata_msgs(pl.r.nodata(), "float", (float)pl.r.nodata());
+  if (int rc = pl.read(&plen, tdio::DT_F32)) return rc;
+  Input ad; std::vector<int32_t> ad8;
+  if (int rc = ad.open(ad8file)) return rc;
+  if (!tdio::compare_rasters(pl.r, pl.path, ad.r, ad.path)) { td::set_error("ad8 grid does not match"); return TD_ERR_ARG; }   // `return 1`, src/LengthArea.cpp:88
+  nodata_msgs(ad.r.nodata(), "int32_t", (int32_t)ad.r.nodata());
+  if (int rc = ad.read(&ad8, tdio::DT_I32)) return rc;
+  const double t1 = now();
+  std::vector<int16_t> ss((size_t)pl.nx * pl.ny);
+  if (int rc = td_lengtharea_host(plen.data(), ad8.data(), ss.data(), pl.nx, pl.ny, p[0], p[1])) {
+    printf("LengthArea device error: %s\n", td_last_error());
+    return rc;
+  }
+  const double t2 = now();
+  printf("Compute time: %f\n", t2 - t1);
+  if (int rc = write_like(ssfile, ad, tdio::DT_I16, (double)(int16_t)-32768, ss)) return rc;
+  const double t3 = now();
+  printf("Read time: %f\nWrite time: %f\nTotal time: %f\nDevice compute time: %f\n", t1 - t0, t3 - t2, t3 - t0, td_last_compute_seconds());
+  return TD_OK;
 } catch (const std::exception& e) {
   td::set_error(std::string("exception: ") + e.what());
   return TD_ERR_IO;

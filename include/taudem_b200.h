@@ -101,7 +101,8 @@ int td_area_host(const float* ang, const float* w /*NULL unless usew*/, float* s
 /* Point-wise consumers of the area rasters (SURVEY.md 8(f) rank 4).  File level = the reference prototypes
  * `int threshold(char* ssafile, char* srcfile, char* maskfile, float thresh, int usemask)` (src/Threshold.cpp:48) and
  * `int twigrid(char* slopefile, char* areafile, char* twifile)` (src/TWI.cpp:47); host-grid and device-strip level like
- * the other tools.  src: int16, nodata -32768; twi: float32, nodata -1 (within 1 float ulp of the reference's logf). */
+ * the other tools.  src: int16, nodata -32768; twi: float32, nodata -1 (the correctly rounded logarithm: one ulp from the
+ * reference's logf exactly where glibc's logf is not correctly rounded; slopearea likewise with powf). */
 /* Sibling of aread8 on the same sweep (SURVEY.md 8(f) rank 3): the largest / smallest value of a grid on the D8 flow paths above
  * each cell.  File level = `int d8flowpathextremeup(char* pfile, char* safile, char* ssafile, int usemax, char* datasrc, char* lyrname,
  * int uselyrname, int lyrno, int useOutlets, int contcheck)` (src/D8flowpathextremeup.cpp:58); ssa: float32, nodata -FLT_MAX. */
@@ -164,7 +165,7 @@ int td_slopearearatio_host(const float* slp, const float* sca, float* sar, int n
  * `int lengtharea(char* plenfile, char* ad8file, char* ssfile, float* p)` (src/LengthArea.cpp:51; p[0] = M, p[1] = y: ss = 1 where
  * ad8 >= M plen^y, ad8 read as 32-bit integers; TD_ERR_ARG when the two grids do not match; the output takes ad8's georeference).
  * peukerdouglas ss: int16, 0 / 1 on every cell, nodata tag -2; lengtharea ss: int16, nodata -32768 where plen < 0.
- * Both bit-exact (lengtharea's power: see pointwise.cu). */
+ * Both bit-exact (lengtharea decides the cells that depend on the last bit of the power with libm's powf: see pointwise.cu). */
 int td_peukerdouglas(const char* felfile, const char* ssfile, const float* p /* w_mid, w_side, w_diag */);
 int td_lengtharea(const char* plenfile, const char* ad8file, const char* ssfile, const float* p /* M, y */);
 int td_peukerdouglas_host(const float* fel, int16_t* ss, int nx, int ny, float fel_nodata, const float* p);
@@ -363,6 +364,9 @@ int td_slopearearatio_dev(td_ctx*, const float* slp, const float* sca, float* sa
  * share()), then td_peukerdouglas_mark_dev (sm -> ss).  fel_nodata: the elevations' nodata value, in both passes.               */
 int td_peukerdouglas_smooth_dev(td_ctx*, const float* fel, float* sm, td_strip s, float fel_nodata, const float* p, void* stream);
 int td_peukerdouglas_mark_dev(td_ctx*, const float* sm, int16_t* ss, td_strip s, float fel_nodata, void* stream);
+/* td_twi_dev, td_slopearea_dev and td_lengtharea_dev synchronise the stream: they read back the number of cells they leave to
+ * the host (a logarithm or power too close to a float midpoint; a length-area decision that depends on the last bit of powf) and
+ * decide those there (pointwise.cu).                                                                                             */
 int td_lengtharea_dev(td_ctx*, const float* plen, const int32_t* ad8, int16_t* ss, td_strip s, float m, float y, void* stream);
 
 /* Peer mode (one process per GPU on one NVSwitch box): every rank exports the IPC handles of the buffers

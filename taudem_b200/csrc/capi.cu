@@ -35,7 +35,7 @@ td_ctx::td_ctx() {
 }
 td_ctx::~td_ctx() {
   node.release(); cnt.release(); lev.release(); mk.release(); listA.release(); listB.release(); listC.release();
-  tileflags.release(); wsched.release(); rowfact.release(); halo.release();
+  tileflags.release(); wsched.release(); rowfact.release(); halo.release(); pend.release();
   if (d_ctr) cudaFree(d_ctr);
   if (h_ctr) cudaFreeHost(h_ctr);
 }
@@ -753,13 +753,15 @@ int td_threshold_dev(td_ctx*, const float* ssa, const float* mask, int16_t* src,
   if (int rc = check_strip(s)) return rc;
   return td::launch_threshold(ssa, mask, src, Strip(s), thresh, ssa_nodata, (cudaStream_t)stream);
 }
-int td_twi_dev(td_ctx*, const float* slp, const float* sca, float* twi, td_strip s, float slp_nodata, float sca_nodata, void* stream) {
+int td_twi_dev(td_ctx* ctx, const float* slp, const float* sca, float* twi, td_strip s, float slp_nodata, float sca_nodata, void* stream) {
   if (int rc = check_strip(s)) return rc;
-  return td::launch_twi(slp, sca, twi, Strip(s), slp_nodata, sca_nodata, (cudaStream_t)stream);
+  if (!ctx) { td::set_error("td_twi_dev: bad arguments"); return TD_ERR_ARG; }
+  return td::launch_twi(slp, sca, twi, Strip(s), slp_nodata, sca_nodata, (cudaStream_t)stream, &ctx->pend);
 }
-int td_slopearea_dev(td_ctx*, const float* slp, const float* sca, float* sa, td_strip s, float m, float n, void* stream) {
+int td_slopearea_dev(td_ctx* ctx, const float* slp, const float* sca, float* sa, td_strip s, float m, float n, void* stream) {
   if (int rc = check_strip(s)) return rc;
-  return td::launch_slopearea(slp, sca, sa, Strip(s), m, n, (cudaStream_t)stream);
+  if (!ctx) { td::set_error("td_slopearea_dev: bad arguments"); return TD_ERR_ARG; }
+  return td::launch_slopearea(slp, sca, sa, Strip(s), m, n, (cudaStream_t)stream, &ctx->pend);
 }
 int td_slopearearatio_dev(td_ctx*, const float* slp, const float* sca, float* sar, td_strip s, float sca_nodata, void* stream) {
   if (int rc = check_strip(s)) return rc;
@@ -836,10 +838,10 @@ int td_peukerdouglas_mark_dev(td_ctx*, const float* sm, int16_t* ss, td_strip s,
   if (!sm || !ss) { td::set_error("td_peukerdouglas_mark_dev: bad arguments"); return TD_ERR_ARG; }
   return td::launch_pd_mark(sm, ss, Strip(s), fel_nodata, (cudaStream_t)stream);
 }
-int td_lengtharea_dev(td_ctx*, const float* plen, const int32_t* ad8, int16_t* ss, td_strip s, float m, float y, void* stream) {
+int td_lengtharea_dev(td_ctx* ctx, const float* plen, const int32_t* ad8, int16_t* ss, td_strip s, float m, float y, void* stream) {
   if (int rc = check_strip(s)) return rc;
-  if (!plen || !ad8 || !ss) { td::set_error("td_lengtharea_dev: bad arguments"); return TD_ERR_ARG; }
-  return td::launch_lengtharea(plen, ad8, ss, Strip(s), m, y, (cudaStream_t)stream);
+  if (!ctx || !plen || !ad8 || !ss) { td::set_error("td_lengtharea_dev: bad arguments"); return TD_ERR_ARG; }
+  return td::launch_lengtharea(plen, ad8, ss, Strip(s), m, y, (cudaStream_t)stream, &ctx->pend);
 }
 int td_peukerdouglas_host(const float* fel, int16_t* ss, int nx, int ny, float fel_nodata, const float* p) {
   if (int rc = need_device()) return rc;

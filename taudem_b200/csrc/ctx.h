@@ -37,6 +37,7 @@ struct td_ctx {
   Buf rows;      // per-row dxc | dyc (host-grid level calls)
   Buf rowfact;   // per-row constants of the flow-direction stencils (rowfact.cuh)
   Buf io[7];     // raster strips of host-grid level calls
+  Buf pend;      // twi, slopearea, lengtharea: the count and list of the cells decided on the host (pointwise.cu)
   // peer mode of the sweeps (neighbour strips' buffers opened through CUDA IPC, see sweep_warp.cu)
   struct PeerInfo { void *cntw = nullptr, *tileflags = nullptr, *dctr = nullptr, *halo_in = nullptr; int qmask = 0, ntx = 0, ny = 0, th = 0, nt = 0, valid = 0, nsh = 1, qshift = 0; };
   PeerInfo peer_up, peer_down;

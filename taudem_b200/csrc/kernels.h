@@ -43,10 +43,15 @@ void sweep_peer_off(td_ctx* ctx);
 int fill_init(const float* dem, const short* mask, float* W, const Strip& s, float nodata, int four, cudaStream_t st);
 int fill_relax(td_ctx* ctx, const float* dem, float* W, const Strip& s, int four, int* changed, cudaStream_t st, bool edges_only = false);
 int launch_threshold(const float* ssa, const float* mask, short* src, const Strip& s, float thresh, float ssa_nodata, cudaStream_t st);
-int launch_slopearea(const float* slp, const float* sca, float* sa, const Strip& s, float m, float n, cudaStream_t st);
+// twi, slopearea and lengtharea synchronise st; pend holds the cells they decide on the host (a context's buffer; nullptr: one
+// allocated for the call, pointwise.cu)
+int launch_slopearea(const float* slp, const float* sca, float* sa, const Strip& s, float m, float n, cudaStream_t st,
+                     td_ctx::Buf* pend = nullptr);
 int launch_slopearearatio(const float* slp, const float* sca, float* sar, const Strip& s, float sca_nodata, cudaStream_t st);
-int launch_twi(const float* slp, const float* sca, float* twi, const Strip& s, float slp_nodata, float sca_nodata, cudaStream_t st);
-int launch_lengtharea(const float* plen, const int* ad8, short* ss, const Strip& s, float m, float y, cudaStream_t st);
+int launch_twi(const float* slp, const float* sca, float* twi, const Strip& s, float slp_nodata, float sca_nodata, cudaStream_t st,
+               td_ctx::Buf* pend = nullptr);
+int launch_lengtharea(const float* plen, const int* ad8, short* ss, const Strip& s, float m, float y, cudaStream_t st,
+                      td_ctx::Buf* pend = nullptr);
 int launch_pd_smooth(const float* fel, float* sm, const Strip& s, float nodata, const float* p /* host: w_mid, w_side, w_diag */, cudaStream_t st);
 int launch_pd_mark(const float* sm, short* ss, const Strip& s, float nodata, cudaStream_t st);
 int launch_mask_ok(const int* mask, float* ok, const Strip& s, int thresh, cudaStream_t st);

@@ -1,6 +1,7 @@
-// TEST INFRASTRUCTURE ONLY — the Peuker-Douglas stencils (k_pd_smooth, k_pd_mark, peuker.cu) and k_lengtharea (pointwise.cu) on the
-// CPU emulation, on one strip or on row strips with the smoothed edge rows exchanged between the two passes like a row-strip
-// caller does.  tests/test_stream_definition.py compares the rasters with the restatements bit for bit.
+// TEST INFRASTRUCTURE ONLY — the Peuker-Douglas stencils (k_pd_smooth, k_pd_mark, peuker.cu) and the point-wise kernels
+// (k_lengtharea with its host resolve, k_threshold, k_twi, k_slopearea, k_slopearearatio: pointwise.cu) on the CPU emulation, the
+// stencils on one strip or on row strips with the smoothed edge rows exchanged between the two passes like a row-strip caller
+// does.  tests/test_stream_definition.py and tests/test_pointwise.py compare the rasters with the restatements cell by cell.
 #include <string>
 #include <vector>
 
@@ -52,16 +53,51 @@ extern "C" int emu_peukerdouglas(const float* fel, short* ss, int nx, int ny, fl
   return 0;
 }
 
-extern "C" int emu_lengtharea(const float* plen, const int* ad8, short* ss, int nx, int ny, float m, float y) {
+// the point-wise kernels on one strip of an nx x ny grid: dense rasters in and out, the padding columns filled with pad
+static Strip one_strip(int nx, int ny) {
   td_strip ts; ts.nx = nx; ts.ny = ny; ts.pitch = (nx + 31) / 32 * 32; ts.has_top = 0; ts.has_bot = 0;
-  const Strip s(ts);
-  std::vector<float> l((size_t)s.cells(), 0.f);
-  std::vector<int> a((size_t)s.cells(), 0);
-  std::vector<short> o((size_t)s.cells(), 0);
-  for (int r = 1; r <= ny; ++r)
-    for (int c = 0; c < nx; ++c) { l[s.idx(r, c)] = plen[(size_t)(r - 1) * nx + c]; a[s.idx(r, c)] = ad8[(size_t)(r - 1) * nx + c]; }
-  if (td::launch_lengtharea(l.data(), a.data(), o.data(), s, m, y, nullptr)) return 1;
-  for (int r = 1; r <= ny; ++r)
-    for (int c = 0; c < nx; ++c) ss[(size_t)(r - 1) * nx + c] = o[s.idx(r, c)];
+  return Strip(ts);
+}
+template <typename T> static std::vector<T> to_strip(const T* g, const Strip& s, T pad) {
+  std::vector<T> v((size_t)s.cells(), pad);
+  if (g)
+    for (int r = 1; r <= s.ny; ++r)
+      for (int c = 0; c < s.nx; ++c) v[s.idx(r, c)] = g[(size_t)(r - 1) * s.nx + c];
+  return v;
+}
+template <typename T> static void from_strip(const std::vector<T>& v, const Strip& s, T* g) {
+  for (int r = 1; r <= s.ny; ++r)
+    for (int c = 0; c < s.nx; ++c) g[(size_t)(r - 1) * s.nx + c] = v[s.idx(r, c)];
+}
+
+static td_ctx::Buf g_pend;
+// n_pend: how many cells the kernel left to the host (the count of the last run)
+extern "C" int emu_lengtharea(const float* plen, const int* ad8, short* ss, int nx, int ny, float m, float y, unsigned* n_pend) {
+  const Strip s = one_strip(nx, ny);
+  std::vector<float> l = to_strip(plen, s, 0.f);
+  std::vector<int> a = to_strip(ad8, s, 0);
+  std::vector<short> o((size_t)s.cells(), 7);
+  if (td::launch_lengtharea(l.data(), a.data(), o.data(), s, m, y, nullptr, &g_pend)) return 1;
+  if (n_pend) *n_pend = *g_pend.as<unsigned>();
+  from_strip(o, s, ss);
+  return 0;
+}
+extern "C" int emu_threshold(const float* ssa, const float* mask, short* src, int nx, int ny, float thresh, float nodata) {
+  const Strip s = one_strip(nx, ny);
+  std::vector<float> v = to_strip(ssa, s, 0.f), mk = to_strip(mask, s, 0.f);
+  std::vector<short> o((size_t)s.cells(), 7);
+  if (td::launch_threshold(v.data(), mask ? mk.data() : nullptr, o.data(), s, thresh, nodata, nullptr)) return 1;
+  from_strip(o, s, src);
+  return 0;
+}
+// which: 0 twi (a, b = the slope's and the area's nodata), 1 slopearea (a, b = m, n), 2 slopearearatio (a = the area's nodata)
+extern "C" int emu_slp_sca(int which, const float* slp, const float* sca, float* out, int nx, int ny, float a, float b) {
+  const Strip s = one_strip(nx, ny);
+  std::vector<float> sl = to_strip(slp, s, 1.f), ar = to_strip(sca, s, 1.f), o((size_t)s.cells(), 7.f);
+  const int rc = which == 0 ? td::launch_twi(sl.data(), ar.data(), o.data(), s, a, b, nullptr, &g_pend)
+               : which == 1 ? td::launch_slopearea(sl.data(), ar.data(), o.data(), s, a, b, nullptr, &g_pend)
+                            : td::launch_slopearearatio(sl.data(), ar.data(), o.data(), s, a, nullptr);
+  if (rc) return 1;
+  from_strip(o, s, out);
   return 0;
 }

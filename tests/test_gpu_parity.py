@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 import flat_cases
+import pointwise_cases as P
 import port
 import sibling_cases
 import taudem_b200 as td
@@ -507,7 +508,8 @@ def test_dinf_conc_lim_and_trans_lim_accumulation(refrun, tmp_path):
 def test_pointwise_consumers_threshold_and_twi(refrun, tmp_path):
     """threshold and twi (SURVEY.md 8(f) rank 4) on the rasters of the path: grid level and our executables against the
     reference executables (oracle/_ref/threshold, oracle/_ref/twi: Threshold.cpp / TWI.cpp compiled unchanged).  src is
-    bit-exact; twi = ln(sca / slp) may differ from glibc's logf in the last bit (<= 1 ulp), with identical nodata masks."""
+    bit-exact; twi = ln(sca / slp) is correctly rounded, so it differs from glibc's logf exactly where logf is not correctly
+    rounded (tests/pointwise_cases.py)."""
     import os
     import subprocess
     dem = synth.punch_holes(synth.gen_dem(300, 380, hurst=0.8, tilt=1.0, seed=31))
@@ -519,11 +521,8 @@ def test_pointwise_consumers_threshold_and_twi(refrun, tmp_path):
     src_ref = R.threshold(ad8, 7.5, mask=mask)
     assert_bits(td.threshold_grid(ad8, 7.5, mask=mask), src_ref, "src -mask")
     twi, ref = td.twi_grid(slp, sca), R.twi(slp, sca)
-    assert np.array_equal(twi == -1.0, ref == -1.0), "twi nodata masks differ"
-    ok = ref != -1.0
-    ulp = np.abs(twi[ok].view(np.int32).astype(np.int64) - ref[ok].view(np.int32).astype(np.int64))
-    assert ulp.max() <= 1, f"twi differs by {ulp.max()} ulp"
-    assert (ulp == 0).mean() > 0.9
+    assert_bits(P.twi(slp, sca), ref, "twi restatement with libm's logf")
+    P.assert_log_pow_contract(twi, P.twi(slp, sca), P.twi(slp, sca, libm=False), "twi")
     # executables on the files the reference run left in tmp_path
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     out = str(tmp_path / "ours_src.tif")
@@ -541,7 +540,8 @@ def test_pointwise_consumers_threshold_and_twi(refrun, tmp_path):
 def test_pointwise_consumers_slopearea_and_slopearearatio(refrun, tmp_path):
     """slopearea and slopearearatio (the other two tools of SURVEY.md 8(f) rank 4): grid level and our executables against the
     reference executables (SlopeArea.cpp / SlopeAreaRatio.cpp compiled unchanged).  sar = slp / sca is bit-exact; sa = slp^m * sca^n
-    is a product of two powf results in the reference (< 1 ulp each): relative 1e-6 with identical nodata masks."""
+    is a product of two powf results in the reference; ours of two correctly rounded powers, so it differs exactly where a powf is
+    not correctly rounded (tests/pointwise_cases.py)."""
     import os
     import subprocess
     dem = synth.punch_holes(synth.gen_dem(260, 420, hurst=0.8, tilt=1.0, seed=37))
@@ -553,10 +553,9 @@ def test_pointwise_consumers_slopearea_and_slopearearatio(refrun, tmp_path):
     for m, n in ((None, None), (0.5, 1.75)):
         ours = td.slopearea_grid(slp, sca) if m is None else td.slopearea_grid(slp, sca, m, n)
         ref = R.slopearea(slp, sca, m, n)
-        assert np.array_equal(ours == -1.0, ref == -1.0), "sa nodata masks differ"
-        ok = ref != -1.0
-        np.testing.assert_allclose(ours[ok], ref[ok], rtol=1e-6, atol=0)
-        assert (ours[ok] == ref[ok]).mean() > 0.9
+        mm, nn = (2.0, 1.0) if m is None else (m, n)
+        assert_bits(P.slopearea(slp, sca, mm, nn), ref, "slopearea restatement with libm's powf")
+        P.assert_log_pow_contract(ours, P.slopearea(slp, sca, mm, nn), P.slopearea(slp, sca, mm, nn, libm=False), f"slopearea {m} {n}")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     out = str(tmp_path / "ours_sa.tif")
     r = subprocess.run([os.path.join(root, "taudem_b200", "bin", "slopearea"), "-slp", str(tmp_path / "slpin.tif"), "-sca", str(tmp_path / "scain.tif"), "-sa", out,

@@ -120,8 +120,8 @@ def test_lengtharea_grid_refuses_a_non_int32_area():
 
 
 # ---------------------------------------------------------------- the kernels on the CPU emulation
-@pytest.fixture(scope="module")
-def emu():
+def build_pd_emu():
+    """tests/emu/pd_driver.cpp with peuker.cu and pointwise.cu on the CPU emulation (also the point-wise kernels' tests)"""
     os.makedirs(test_emu.BUILD, exist_ok=True)
     incs = [test_emu._transform("peuker", 2), test_emu._transform("pointwise", 7)]
     so = os.path.join(test_emu.BUILD, "libemu_pd.so")
@@ -133,8 +133,15 @@ def emu():
     lib = C.CDLL(so)
     P = C.c_void_p
     lib.emu_peukerdouglas.argtypes = [P, P, C.c_int, C.c_int, C.c_float, P, C.c_int, P]
-    lib.emu_lengtharea.argtypes = [P, P, P, C.c_int, C.c_int, C.c_float, C.c_float]
+    lib.emu_lengtharea.argtypes = [P, P, P, C.c_int, C.c_int, C.c_float, C.c_float, P]
+    lib.emu_threshold.argtypes = [P, P, P, C.c_int, C.c_int, C.c_float, C.c_float]
+    lib.emu_slp_sca.argtypes = [C.c_int, P, P, P, C.c_int, C.c_int, C.c_float, C.c_float]
     return lib
+
+
+@pytest.fixture(scope="module")
+def emu():
+    return build_pd_emu()
 
 
 def _emu_pd(lib, fel, weights=(0.4, 0.1, 0.05), strips=None):
@@ -205,5 +212,5 @@ def test_emulated_lengtharea_matches_the_restatement(emu):
             mm, yy = (0.03, 1.3) if m is None else (m, y)
             ss = np.empty(pl.shape, np.int16)
             p = np.ascontiguousarray(pl, np.float32)
-            assert emu.emu_lengtharea(p.ctypes.data, ai.ctypes.data, ss.ctypes.data, pl.shape[1], pl.shape[0], mm, yy) == 0
+            assert emu.emu_lengtharea(p.ctypes.data, ai.ctypes.data, ss.ctypes.data, pl.shape[1], pl.shape[0], mm, yy, None) == 0
             assert_bits(ss, restate.lengtharea(pl, a, m, y), f"{pl.shape} {m} {y}")

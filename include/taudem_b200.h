@@ -170,6 +170,14 @@ int td_peukerdouglas(const char* felfile, const char* ssfile, const float* p /* 
 int td_lengtharea(const char* plenfile, const char* ad8file, const char* ssfile, const float* p /* M, y */);
 int td_peukerdouglas_host(const float* fel, int16_t* ss, int nx, int ny, float fel_nodata, const float* p);
 int td_lengtharea_host(const float* plen, const int32_t* ad8, int16_t* ss, int nx, int ny, float m, float y);
+/* slopeavedown: the D8 slope averaged over the downslope distance dn (the downslope gradient index).  File level = `int sloped(char*
+ * pfile, char* felfile, char* slpdfile, double dn)` (src/SlopeAveDown.cpp:59; TD_ERR_MISMATCH when fel and p differ in size).
+ * slpd: float32, nodata MISSINGFLOAT, the georeference of p.  Host-grid level: dxc / dyc = per-row cell sizes (the distances),
+ * dx / dy = the header's cell sizes (niter = dn / min(dx, dy) + 1 passes).  TD_ERR_ARG when dn is not finite or niter does not fit
+ * an int.  Bit-exact; stops early, with the same result, once a pass changes nothing. */
+int td_sloped(const char* pfile, const char* felfile, const char* slpdfile, double dn);
+int td_slopeavedown_host(const float* fel, const int16_t* p, float* slpd, int nx, int ny, float fel_nodata, int16_t p_nodata, const double* dxc,
+                         const double* dyc, double dx, double dy, double dn);
 
 /* aread8 + areadinf of one DEM in one call (no weights, no outlets), the host<->device copies overlapped with the kernels
  * on three streams: p in -> aread8 || ang in -> areadinf || ad8 out -> sca out.  Same results as the two calls above.
@@ -368,6 +376,20 @@ int td_peukerdouglas_mark_dev(td_ctx*, const float* sm, int16_t* ss, td_strip s,
  * the host (a logarithm or power too close to a float midpoint; a length-area decision that depends on the last bit of powf) and
  * decide those there (pointwise.cu).                                                                                             */
 int td_lengtharea_dev(td_ctx*, const float* plen, const int32_t* ad8, int16_t* ss, td_strip s, float m, float y, void* stream);
+/* slopeavedown on a strip (slopeavedown.cu).  First the D8 dependency stencil and sweep of p on the same context (td_aread8_deps_dev,
+ * then td_aread8_sweep_dev or the row-strip / peer protocol): the cells the sweep evaluates are the cells the reference's queue
+ * processes.  Then td_slopeavedown_init_dev (p and fel with valid halo rows) writes code (one byte per strip cell), both state
+ * buffers ed_dd0 and ed_dd1 (two floats per strip cell: the elevation and the distance carried up from downslope, the halo rows
+ * included) and sd (MISSINGFLOAT).  Each td_slopeavedown_pass_dev is one of the reference's passes: state in -> state out (swap the
+ * two between passes), sd updated in place; *changed (host) = whether any bit of the state or sd changed (it synchronises the
+ * stream).  On row strips the caller copies the first / last owned rows of the pass's output state (8 bytes per cell) into the
+ * neighbours' halo rows between passes (the reference's ed->share(); dd->share()).  dist: device table of the strip's own rows,
+ * dist[8 * (row - 1) + k - 1] = (float)sqrt(d1[k]^2 dxc^2 + d2[k]^2 dyc^2).  td_slopeavedown_niter: the reference's pass count. */
+int td_slopeavedown_init_dev(td_ctx*, const int16_t* p, const float* fel, uint8_t* code, float* ed_dd0, float* ed_dd1, float* sd, td_strip s,
+                             int16_t p_nodata, float fel_nodata, void* stream);
+int td_slopeavedown_pass_dev(td_ctx*, const uint8_t* code, const float* fel, const float* ed_dd_in, float* ed_dd_out, float* sd, td_strip s,
+                             const float* dist, double dn, int* changed, void* stream);
+int td_slopeavedown_niter(double dn, double dx, double dy, int* niter);
 
 /* Peer mode (one process per GPU on one NVSwitch box): every rank exports the IPC handles of the buffers
  * its neighbours write (counts, tile scheduler, halo areas, rank 0 also the global pending counter), opens

@@ -59,7 +59,7 @@ def main():
     sca = s.empty(torch.float32)
     run("k_deps_dinf", 4, lambda: T.areadinf_deps(s, ang, sca, dxc, dyc))
     run("k_deps_dinf (+7 scratch)", 11, lambda: T.areadinf_deps(s, ang, sca, dxc, dyc))
-    if only is not None and not (only & {"k_threshold", "k_twi", "k_slopearea", "k_slopearearatio", "k_pd_smooth", "k_pd_mark", "k_lengtharea"}):
+    if only is not None and not (only & {"k_threshold", "k_twi", "k_slopearea", "k_slopearearatio", "k_pd_smooth", "k_pd_mark", "k_lengtharea", "k_sad_pass"}):
         print(json.dumps({"n": n, "hbm_peak_gbs": peak, "kernels": out}))
         return
     # point-wise consumers on the rasters of the path
@@ -77,6 +77,15 @@ def main():
     run("k_pd_mark", B(sm, ss), lambda: T.l.td_peukerdouglas_mark_dev(T.ctx, _p(sm), _p(ss), s.c, C.c_float(-3.0e38), T._stream()))
     ad8i = ad8.round().to(torch.int32)
     run("k_lengtharea", B(ad8, ad8i, ss), lambda: T.l.td_lengtharea_dev(T.ctx, _p(ad8), _p(ad8i), _p(ss), s.c, C.c_float(0.03), C.c_float(1.3), T._stream()))
+    # slopeavedown: the D8 sweep's counts mark the processed cells, then one pass at dn = 50 (the first pass: no slope is due yet, so
+    # per cell the code byte, the state pair in and out and the slope's nodata test; sd is written in place only where a slope is due)
+    T.aread8_deps(s, p, ad8); T.aread8_sweep(s, ad8)
+    code = s.empty(torch.uint8); sd = s.empty(torch.float32)
+    st0 = torch.empty((s.ny + 2, 2 * s.pitch), dtype=torch.float32, device="cuda"); st1 = torch.empty_like(st0)
+    T.l.td_slopeavedown_init_dev(T.ctx, _p(p), _p(fel), _p(code), _p(st0), _p(st1), _p(sd), s.c, -32768, C.c_float(-3.0e38), T._stream())
+    dist = torch.tensor([30.0, 900.0 ** 0.5 * 2 ** 0.5] * 4, dtype=torch.float32).repeat(s.ny).cuda()
+    run("k_sad_pass", 21, lambda: T.l.td_slopeavedown_pass_dev(T.ctx, _p(code), _p(fel), _p(st0), _p(st1), _p(sd), s.c, _p(dist), C.c_double(50.0), None,
+                                                               T._stream()))
     print(json.dumps({"n": n, "hbm_peak_gbs": peak, "kernels": out}))
 
 

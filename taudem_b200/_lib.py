@@ -68,6 +68,11 @@ SIGNATURES = {
     "td_peukerdouglas_smooth_dev": (_I, [_P, _P, _P, Strip, _F, _P, _P]),
     "td_peukerdouglas_mark_dev": (_I, [_P, _P, _P, Strip, _F, _P]),
     "td_lengtharea_dev": (_I, [_P, _P, _P, _P, Strip, _F, _F, _P]),
+    "td_sloped": (_I, [_S, _S, _S, _D]),
+    "td_slopeavedown_host": (_I, [_P, _P, _P, _I, _I, _F, C.c_int16, _P, _P, _D, _D, _D]),
+    "td_slopeavedown_init_dev": (_I, [_P, _P, _P, _P, _P, _P, _P, Strip, C.c_int16, _F, _P]),
+    "td_slopeavedown_pass_dev": (_I, [_P, _P, _P, _P, _P, _P, Strip, _P, _D, _P, _P]),
+    "td_slopeavedown_niter": (_I, [_D, _D, _D, _P]),
     "td_nameadd": (_I, [_S, _S, _S]),
     "td_raster_info": (_I, [_S] + [_P] * 9),
     "td_raster_read": (_I, [_S, _I, _P, _I, _I]),

@@ -304,6 +304,24 @@ def lengtharea_grid(plen, ad8, m=0.03, y=1.3):
     return ss
 
 
+def slopeavedown_grid(fel, p, dn=50.0, dx=30.0, dy=30.0, nodata=float(FEL_NODATA), p_nodata=int(MISSINGSHORT), dxc=None, dyc=None):
+    """D8 slope averaged over the downslope distance dn (td_slopeavedown_host; src/SlopeAveDown.cpp:59-330): for every cell the
+    aread8 queue reaches, (fel - the elevation at the end of its flow path dn further down) / that path's length, float32, nodata
+    MISSINGFLOAT.  dx / dy: the header's cell sizes, from which the pass count dn / min(dx, dy) + 1 comes; dxc / dyc: per-row cell
+    sizes for the distances (default dx / dy on every row)."""
+    fel = _grid(fel, np.float32)
+    p = _grid(p, np.int16)
+    ny, nx = fel.shape
+    if p.shape != fel.shape:
+        raise ValueError("slopeavedown_grid: fel and p differ in shape")
+    dxc = _rows(dx if dxc is None else dxc, ny)
+    dyc = _rows(dy if dyc is None else dyc, ny)
+    slpd = np.empty((ny, nx), np.float32)
+    check(lib().td_slopeavedown_host(_ptr(fel), _ptr(p), _ptr(slpd), nx, ny, np.float32(nodata), int(p_nodata), _ptr(dxc), _ptr(dyc), float(dx),
+                                     float(dy), float(dn)))
+    return slpd
+
+
 def contributing_areas_grid(p, ang, p_nodata=int(MISSINGSHORT), ang_nodata=float(MISSINGFLOAT), dx=30.0, dy=30.0, contcheck=True, out_ad8=None, out_sca=None):
     """aread8 + areadinf of one DEM in one call, copies overlapped with the kernels (td_contributing_areas_host)."""
     p = _grid(p, np.int16); ang = _grid(ang, np.float32)

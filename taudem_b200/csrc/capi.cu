@@ -879,6 +879,82 @@ int td_lengtharea_host(const float* plen, const int32_t* ad8, int16_t* ss, int n
   return TD_OK;
 }
 
+// ---- slopeavedown (slopeavedown.cu): the D8 sweep marks the cells the reference's queue processes, then the passes
+// niter = (int)(dn / min(dx, dy) + 1) (src/SlopeAveDown.cpp:172); TD_ERR_ARG where the reference's conversion is undefined
+int td_slopeavedown_niter(double dn, double dx, double dy, int* niter) {
+  const double v = dn / std::min(dx, dy) + 1;
+  if (!niter || !isfinite(dn) || !(v > -2147483649.0 && v < 2147483648.0)) {
+    td::set_error("slopeavedown: dn / min(dx, dy) + 1 is not a finite number that fits an int");
+    return TD_ERR_ARG;
+  }
+  *niter = (int)v;
+  return TD_OK;
+}
+int td_slopeavedown_init_dev(td_ctx* ctx, const int16_t* p, const float* fel, uint8_t* code, float* ed_dd0, float* ed_dd1, float* sd, td_strip s,
+                             int16_t p_nodata, float fel_nodata, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  if (!ctx || !p || !fel || !code || !ed_dd0 || !ed_dd1 || !sd || ed_dd0 == ed_dd1 || !ctx->cnt.p || ctx->sweep_dinf) {
+    td::set_error("td_slopeavedown_init_dev: bad arguments (the D8 dependency stencil and sweep of p come first, on this context)");
+    return TD_ERR_ARG;
+  }
+  return td::launch_sad_init(p, ctx->cnt.as<unsigned char>(), fel, code, ed_dd0, ed_dd1, sd, Strip(s), p_nodata, fel_nodata, (cudaStream_t)stream);
+}
+int td_slopeavedown_pass_dev(td_ctx* ctx, const uint8_t* code, const float* fel, const float* ed_dd_in, float* ed_dd_out, float* sd, td_strip s,
+                             const float* dist, double dn, int* changed, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  if (!ctx || !code || !fel || !ed_dd_in || !ed_dd_out || !sd || !dist || ed_dd_in == ed_dd_out) {
+    td::set_error("td_slopeavedown_pass_dev: bad arguments");
+    return TD_ERR_ARG;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  int* d_flag = reinterpret_cast<int*>(ctx->d_ctr + 36);
+  TD_CUDA(cudaMemsetAsync(d_flag, 0, sizeof(int), st));
+  if (int rc = td::launch_sad_pass(code, fel, ed_dd_in, ed_dd_out, sd, dist, Strip(s), dn, d_flag, st)) return rc;
+  if (changed) {
+    TD_CUDA(cudaMemcpyAsync(ctx->h_ctr + 36, d_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    TD_CUDA(cudaStreamSynchronize(st));
+    *changed = *reinterpret_cast<const int*>(ctx->h_ctr + 36) != 0;
+  }
+  return TD_OK;
+}
+// src/SlopeAveDown.cpp:59-330 on one strip: the D8 sweep, then at most niter passes (none after the first that changes nothing)
+int td_slopeavedown_host(const float* fel, const int16_t* p, float* slpd, int nx, int ny, float fel_nodata, int16_t p_nodata, const double* dxc,
+                         const double* dyc, double dx, double dy, double dn) {
+  if (int rc = need_device()) return rc;
+  if (!fel || !p || !slpd || !dxc || !dyc || nx <= 0 || ny <= 0) { td::set_error("td_slopeavedown_host: bad arguments"); return TD_ERR_ARG; }
+  int niter = 0;
+  if (int rc = td_slopeavedown_niter(dn, dx, dy, &niter)) return rc;
+  td_ctx* ctx = default_ctx();
+  const td_strip s = host_strip(nx, ny);
+  const size_t n = (size_t)Strip(s).cells();
+  cudaStream_t st = 0;
+  TD_CUDA(ctx->io[0].ensure(n * 2)); TD_CUDA(ctx->io[1].ensure(n * 4)); TD_CUDA(ctx->io[2].ensure(n * 4));
+  TD_CUDA(ctx->io[3].ensure(n)); TD_CUDA(ctx->io[4].ensure(n * 8)); TD_CUDA(ctx->io[5].ensure(n * 8));
+  int16_t* d_p = ctx->io[0].as<int16_t>(); float* d_fel = ctx->io[1].as<float>();
+  float* d_sd = ctx->io[2].as<float>();                 // the sweep's area scratch first, then the slopes
+  uint8_t* d_code = ctx->io[3].as<uint8_t>();
+  float* d_state[2] = {ctx->io[4].as<float>(), ctx->io[5].as<float>()};
+  std::vector<float> dist((size_t)ny * 8);
+  td::gridnet_dist_table(dxc, dyc, ny, dist.data());
+  TD_CUDA(ctx->rows.ensure(sizeof(float) * dist.size()));
+  float* d_dist = ctx->rows.as<float>();
+  TD_CUDA(cudaMemcpyAsync(d_dist, dist.data(), sizeof(float) * dist.size(), cudaMemcpyHostToDevice, st));
+  TD_CUDA(h2d(d_p, p, s, st)); TD_CUDA(h2d(d_fel, fel, s, st));
+  Timer t; t.start(st);
+  if (int rc = td_aread8_deps_dev(ctx, d_p, d_sd, s, p_nodata, st)) return rc;
+  if (int rc = td_aread8_sweep_dev(ctx, nullptr, d_sd, s, 0.f, 0, 0, st)) return rc;
+  if (int rc = td_slopeavedown_init_dev(ctx, d_p, d_fel, d_code, d_state[0], d_state[1], d_sd, s, p_nodata, fel_nodata, st)) return rc;
+  for (int it = 0; it < niter; ++it) {
+    int changed = 0;
+    if (int rc = td_slopeavedown_pass_dev(ctx, d_code, d_fel, d_state[it & 1], d_state[(it + 1) & 1], d_sd, s, d_dist, dn, &changed, st)) return rc;
+    if (!changed) break;                               // a fixed point: the remaining passes would change nothing
+  }
+  td::set_compute_seconds(t.stop(st));
+  TD_CUDA(d2h(slpd, d_sd, s, st));
+  TD_CUDA(cudaStreamSynchronize(st));
+  return TD_OK;
+}
+
 // aread8 + areadinf of one DEM in ONE call with the copies overlapped with the kernels: three streams — host -> device (p, then
 // ang), compute (aread8 as soon as p has arrived, areadinf as soon as ang has and aread8 is done), device -> host (ad8 while
 // areadinf runs, then sca).  Same kernels, same results as td_aread8_host followed by td_area_host (no weights, no outlets).

@@ -1,5 +1,5 @@
 // Command line front ends: pitremove, d8flowdir, dinfflowdir, aread8, areadinf (+ the point-wise consumers threshold, twi, slopearea, slopearearatio,
-// the sibling sweep tools and the stream definitions peukerdouglas and lengtharea).
+// the sibling sweep tools, the stream definitions peukerdouglas and lengtharea, and slopeavedown).
 // Same flags, same two invocation styles and the same "print usage and exit(0)" error
 // behaviour as the reference mains (src/PitRemovemn.cpp:48-172, src/D8FlowDirmn.cpp:49-146,
 // src/DinfFlowDirmn.cpp:54-147, src/aread8mn.cpp:49-193, src/areadinfmn.cpp:49-178);
@@ -18,7 +18,8 @@ static int done() { fflush(stdout); fflush(stderr); _exit(0); return 0; }
 
 struct Opt {
   const char* flag;
-  int kind;        // 0 = file name, 1 = switch, 2 = integer, 3 = float (ival points to a float), 4 = two floats, 5 = three floats
+  int kind;        // 0 = file name, 1 = switch, 2 = integer, 3 = float (ival points to a float), 4 = two floats, 5 = three floats,
+                   // 6 = double (ival points to a double)
   char* sval;      // kind 0
   int* ival;       // kind 1 (set to `set`) / kind 2 (parsed) / kind 0 (set to `set` when given, may be NULL)
   int set;
@@ -44,6 +45,7 @@ static void parse(int argc, char** argv, Opt* opts, int nopts) {
     if (argc <= i) usage(argv[0]);
     if (o->kind == 0) { strncpy(o->sval, argv[i], MAXLN - 1); o->sval[MAXLN - 1] = 0; if (o->ival) *o->ival = o->set; }
     else if (o->kind == 3) sscanf(argv[i], "%f", (float*)o->ival);
+    else if (o->kind == 6) sscanf(argv[i], "%lf", (double*)o->ival);
     else if (o->kind == 4) { if (argc <= i + 1) usage(argv[0]); sscanf(argv[i], "%f", (float*)o->ival); i++; sscanf(argv[i], "%f", (float*)o->ival + 1); }
     else if (o->kind == 5) { if (argc <= i + 2) usage(argv[0]); for (int k = 0; k < 3; ++k, ++i) sscanf(argv[i], "%f", (float*)o->ival + k); i--; }
     else sscanf(argv[i], "%d", o->ival);
@@ -487,6 +489,34 @@ int main(int argc, char** argv) {
   if (argc == 2) { td_nameadd(plen, argv[1], "plen"); td_nameadd(ad8, argv[1], "ad8"); td_nameadd(ss, argv[1], "ss"); }
   int err = td_lengtharea(plen, ad8, ss, par);
   if (err != 0) printf("Length Area Error %d\n", err);
+  return done();
+}
+#elif defined(TOOL_slopeavedown)
+// src/SlopeAveDownmn.cpp:49-145 (the reference's usage text, typos included; -dn is read with %lf, default 50)
+static void usage(const char* prog) {
+  printf("Simple Usage:\n %s <basefilename>\n", prog);
+  printf("Usage with specific file names:\n %s -p <pfile>\n", prog);
+  printf("-fel <felfile> -slpd <slpdfile> -dn <dn>\n");
+  printf("<basefilename> is the name of the base digital elevation model\n");
+  printf("<pfile> is the D8 flow direction input file.\n");
+  printf("<felfile> is the pit filled or carved elevation input file.\n");
+  printf("<slpdfile> is the output D8 slope distance averaged grid file.\n");
+  printf("<dn is the optional user selected downslope distance.\n");
+  printf("The following are appended to the file names\n");
+  printf("before the files are opened:\n");
+  printf("fel   pit filled or carved elevation grid (input)\n");
+  printf("p   D-infinity flow direction grid (Input)\n");
+  printf("slpd   avalanche source site grod (input)\n");
+  exit(0);
+}
+int main(int argc, char** argv) {
+  static char p[MAXLN], fel[MAXLN], slpd[MAXLN];
+  double dn = 50.0;
+  Opt opts[] = {{"-fel", 0, fel, NULL, 0}, {"-p", 0, p, NULL, 0}, {"-slpd", 0, slpd, NULL, 0}, {"-dn", 6, NULL, (int*)&dn, 0}};
+  parse(argc, argv, opts, 4);
+  if (argc == 2) { td_nameadd(fel, argv[1], "fel"); td_nameadd(p, argv[1], "p"); td_nameadd(slpd, argv[1], "slpd"); }
+  int err = td_sloped(p, fel, slpd, dn);
+  if (err != 0) printf("sloped error %d\n", err);
   return done();
 }
 #else

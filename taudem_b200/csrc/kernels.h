@@ -54,6 +54,11 @@ int launch_lengtharea(const float* plen, const int* ad8, short* ss, const Strip&
                       td_ctx::Buf* pend = nullptr);
 int launch_pd_smooth(const float* fel, float* sm, const Strip& s, float nodata, const float* p /* host: w_mid, w_side, w_diag */, cudaStream_t st);
 int launch_pd_mark(const float* sm, short* ss, const Strip& s, float nodata, cudaStream_t st);
+// slopeavedown.cu: s0 / s1 = the two (ed, dd) state buffers (float2 per strip cell)
+int launch_sad_init(const short* p, const unsigned char* cnt, const float* fel, unsigned char* code, float* s0, float* s1, float* sd,
+                    const Strip& s, short p_nodata, float fel_nodata, cudaStream_t st);
+int launch_sad_pass(const unsigned char* code, const float* fel, const float* src, float* dst, float* sd, const float* dist, const Strip& s,
+                    double dn, int* changed, cudaStream_t st);
 int launch_mask_ok(const int* mask, float* ok, const Strip& s, int thresh, cudaStream_t st);
 int launch_gord_finish(const float* g, const short* p, const float* ok, const unsigned short* node, short* gord, const Strip& s, short p_nodata,
                        int outlets, cudaStream_t st);

@@ -1,5 +1,6 @@
 // Multi-GPU contributing area behind the executables: `TAUDEM_B200_GPUS=N aread8 ...` / `areadinf ...`, and the same for the five
-// sibling sweep tools (d8flowpathextremeup, gridnet, dinfdecayaccum, dinfconclimaccum, dinftranslimaccum: sibling_worker).
+// sibling sweep tools (d8flowpathextremeup, gridnet, dinfdecayaccum, dinfconclimaccum, dinftranslimaccum: sibling_worker), and
+// slopeavedown, whose passes follow its D8 sweep there.
 //
 // reference: the callers' contract is `mpiexec -n N aread8` (src/aread8.cpp:57,100: MPI_Init, one row strip per rank,
 // src/linearpart.h:160-200 the partition, src/aread8.cpp:280-304 the border exchange + ringTerm loop).  Here the
@@ -261,7 +262,8 @@ void worker(const MgpuJob& J, Shared* S, char* extra, int rank, int world) {
   cudaFree(d_dir); cudaFree(d_out); cudaFree(d_halo); cudaFree(d_w); cudaFree(d_dx);
 }
 
-// ---- the five sibling sweep tools on row strips (MgpuSibJob): the same ranks, strips and boundary modes as aread8 / areadinf
+// ---- the five sibling sweep tools and slopeavedown on row strips (MgpuSibJob): the same ranks, strips and boundary modes as
+//      aread8 / areadinf
 void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int world) {
   int ndev = 0;
   MG_CUDA(cudaGetDeviceCount(&ndev));
@@ -271,7 +273,7 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
   cudaStream_t st;
   MG_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
 
-  const bool dinf = J.tool >= MgpuSibJob::DECAY;
+  const bool dinf = J.tool >= MgpuSibJob::DECAY && J.tool <= MgpuSibJob::TRANSLIM;
   tdio::Raster in;
   std::string err;
   if (!in.open(J.dirfile, &err)) throw Fail{"open " + std::string(J.dirfile) + ": " + err};
@@ -286,9 +288,9 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
   MG_CUDA(cudaMalloc(&d_dir, cells * tdio::dtype_bytes(dt)));
   load_strip(in, dt, d_dir, nx, s.pitch, row0, ny, total_ny, st);
   // the further inputs, each with its halo rows (MgpuSibJob::in)
-  static const tdio::DType in_type[5][3] = {{tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}, {tdio::DT_I32, tdio::DT_F32, tdio::DT_F32},
+  static const tdio::DType in_type[6][3] = {{tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}, {tdio::DT_I32, tdio::DT_F32, tdio::DT_F32},
                                             {tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}, {tdio::DT_F32, tdio::DT_F32, tdio::DT_I16},
-                                            {tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}};
+                                            {tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}, {tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}};
   tdio::Raster rin[3];
   void* d_in[3] = {nullptr, nullptr, nullptr};
   float nd[3] = {0.f, 0.f, 0.f};
@@ -301,6 +303,7 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
   }
   // the travelling value, the other outputs, gridnet's mask grid / distances / orders, the halo counts
   float *d_val = nullptr, *d_dep = nullptr, *d_co = nullptr, *d_ok = nullptr, *d_dist = nullptr; int16_t* d_g = nullptr; int* d_halo = nullptr;
+  uint8_t* d_code = nullptr; float* d_state[2] = {nullptr, nullptr};                      // slopeavedown
   double* d_dx = nullptr;
   MG_CUDA(cudaMalloc(&d_val, cells * 4));
   MG_CUDA(cudaMalloc(&d_halo, sizeof(int) * 4 * (size_t)s.pitch));        // halo_out (2 pitch) + the received decrements (2 pitch)
@@ -310,9 +313,11 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
   }
   std::vector<double> dxc, dyc;
   in.cell_sizes(&dxc, &dyc);
-  if (J.tool == MgpuSibJob::GRIDNET) {
-    if (J.in[0]) MG_CUDA(cudaMalloc(&d_ok, cells * 4));
-    MG_CUDA(cudaMalloc(&d_g, cells * 2));
+  if (J.tool == MgpuSibJob::GRIDNET || J.tool == MgpuSibJob::SLOPEAVEDOWN) {
+    if (J.tool == MgpuSibJob::GRIDNET) {
+      if (J.in[0]) MG_CUDA(cudaMalloc(&d_ok, cells * 4));
+      MG_CUDA(cudaMalloc(&d_g, cells * 2));
+    }
     std::vector<float> dist((size_t)ny * 8);
     gridnet_dist_table(dxc.data() + row0, dyc.data() + row0, ny, dist.data());       // this strip's own rows
     MG_CUDA(cudaMalloc(&d_dist, sizeof(float) * dist.size()));
@@ -378,6 +383,36 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
       one_sweep([&]() { MG_TD(td_dinfconclimaccum_sweep_run_dev(ctx, ang, f0, f1, (const int16_t*)d_in[2], d_val, s, nd[0], nd[1], J.csol, J.contcheck, d_dx,
                                                                 d_halo, st)); }, nullptr);
       break;
+    case MgpuSibJob::SLOPEAVEDOWN: {
+      // the D8 sweep marks the cells the reference's queue processes; then the passes, each followed by the exchange of the state's
+      // edge rows (ed->share(); dd->share(), src/SlopeAveDown.cpp:266-267) and an all-reduce of "anything changed"
+      MG_TD(td_aread8_deps_dev(ctx, (const int16_t*)d_dir, d_val, s, p_nd, st));
+      one_sweep([&]() { MG_TD(td_aread8_sweep_run_dev(ctx, nullptr, d_val, s, 0.f, 0, 0, d_halo, st)); }, nullptr);
+      MG_CUDA(cudaMalloc(&d_code, cells));
+      for (float*& b : d_state) MG_CUDA(cudaMalloc(&b, cells * 8));
+      MG_TD(td_slopeavedown_init_dev(ctx, (const int16_t*)d_dir, f0, d_code, d_state[0], d_state[1], d_val, s, p_nd, nd[0], st));
+      const RoundBuf R{extra, s.pitch};
+      const size_t rb = (size_t)s.pitch * 8;                  // one row of the state; R.row(r, 0..1) and R.row(r, 2..3) hold two
+      for (int it = 0; it < J.niter; ++it) {
+        float* out = d_state[(it + 1) & 1];
+        int changed = 0;
+        MG_TD(td_slopeavedown_pass_dev(ctx, d_code, f0, d_state[it & 1], out, d_val, s, d_dist, J.dn, &changed, st));
+        MG_CUDA(cudaMemcpy(R.row(rank, 0), (const char*)out + rb, rb, cudaMemcpyDeviceToHost));
+        MG_CUDA(cudaMemcpy(R.row(rank, 2), (const char*)out + rb * (size_t)ny, rb, cudaMemcpyDeviceToHost));
+        S->red[rank][0] = (unsigned long long)changed;
+        MG_BAR();
+        unsigned long long any = 0;
+        for (int r = 0; r < world; ++r) any += S->red[r][0];
+        // (on st, so that the next pass is ordered after them)
+        if (rank > 0) MG_CUDA(cudaMemcpyAsync(out, R.row(rank - 1, 2), rb, cudaMemcpyHostToDevice, st));
+        if (rank < world - 1) MG_CUDA(cudaMemcpyAsync((char*)out + rb * (size_t)(ny + 1), R.row(rank + 1, 0), rb, cudaMemcpyHostToDevice, st));
+        MG_CUDA(cudaStreamSynchronize(st));
+        ++rounds;
+        MG_BAR();
+        if (any == 0) break;                                  // no rank changed anything: the remaining passes would not either
+      }
+      break;
+    }
     default:
       MG_TD(td_dinftranslimaccum_deps_dev(ctx, ang, d_val, d_dep, d_co, s, a_nd, d_dx, d_dx + ny, st));
       one_sweep([&]() { MG_TD(td_dinftranslimaccum_sweep_run_dev(ctx, ang, f0, f1, f2, d_val, d_dep, d_co, s, nd[0], nd[1], nd[2], J.contcheck, d_dx,
@@ -394,6 +429,7 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
   }
   td_ctx_destroy(ctx);
   cudaFree(d_dir); cudaFree(d_val); cudaFree(d_dep); cudaFree(d_co); cudaFree(d_ok); cudaFree(d_dist); cudaFree(d_g); cudaFree(d_halo); cudaFree(d_dx);
+  cudaFree(d_code); cudaFree(d_state[0]); cudaFree(d_state[1]);
   for (void* p : d_in) cudaFree(p);
 }
 
@@ -636,7 +672,7 @@ int mgpu_area(const MgpuJob& J, int world, double* compute_seconds, int* rounds)
 int mgpu_sibling(const MgpuSibJob& J, int world, double* compute_seconds, int* rounds) {
   if (world < 2 || world > MAXR) { set_error("mgpu_sibling: between 2 and 64 ranks"); return TD_ERR_ARG; }
   if (J.ny < world) { set_error("mgpu_sibling: fewer rows than ranks"); return TD_ERR_ARG; }
-  if (J.tool < MgpuSibJob::EXTREMEUP || J.tool > MgpuSibJob::TRANSLIM || !J.out[0]) { set_error("mgpu_sibling: bad job"); return TD_ERR_ARG; }
+  if (J.tool < MgpuSibJob::EXTREMEUP || J.tool > MgpuSibJob::SLOPEAVEDOWN || !J.out[0]) { set_error("mgpu_sibling: bad job"); return TD_ERR_ARG; }
   const int pitch = td_pitch_for(J.nx);
   return run_ranks("mgpu_sibling", world, RoundBuf::bytes(pitch) * (size_t)world,
                    [&](Shared* S, char* extra, int r) { sibling_worker(J, S, extra, r, world); }, compute_seconds, rounds, nullptr);

@@ -30,13 +30,15 @@ struct MgpuFlowJob {
 //   DECAY      dinfdecayaccum       in: dm, w              out: dsca
 //   CONCLIM    dinfconclimaccum     in: dm, q, dg (int16)  out: ctpt
 //   TRANSLIM   dinftranslimaccum    in: tsup, tc, cs       out: tla, tdep, ctpt (with cs)
+//   SLOPEAVEDOWN  slopeavedown      in: fel                out: slpd (the D8 sweep of p, then niter passes at dn)
 struct MgpuSibJob {
-  enum { EXTREMEUP = 0, GRIDNET, DECAY, CONCLIM, TRANSLIM };
+  enum { EXTREMEUP = 0, GRIDNET, DECAY, CONCLIM, TRANSLIM, SLOPEAVEDOWN };
   int tool = EXTREMEUP;
   const char* dirfile = nullptr;              // p (D8 tools) or ang
   const char* in[3] = {nullptr, nullptr, nullptr};
   int usemax = 1, contcheck = 1, thresh = 0;
   float csol = 0.f;
+  double dn = 0.; int niter = 0;              // slopeavedown
   int nx = 0, ny = 0;
   void* out[3] = {nullptr, nullptr, nullptr};
 };

@@ -940,4 +940,48 @@ int td_lengtharea(const char* plenfile, const char* ad8file, const char* ssfile,
   return TD_ERR_IO;
 }
 
+// src/SlopeAveDown.cpp:59-330: fel and p in, slpd out (float32, nodata MISSINGFLOAT, the georeference of p).  The distances use fel's
+// per-row cell sizes; niter uses its header cell sizes, dxA / dyA = |dxc| / |dyc| of the middle row (src/tiffIO.cpp:155).
+// TAUDEM_B200_GPUS=N runs it on N row strips.
+int td_sloped(const char* pfile, const char* felfile, const char* slpdfile, double dn) try {
+  printf("SlopeAveDown version %s\n", td_version());
+  fflush(stdout);
+  const double t0 = now();
+  Input z;
+  if (int rc = z.open(felfile)) return rc;
+  nodata_msgs(z.r.nodata(), "float", (float)z.r.nodata());
+  Input p;
+  if (int rc = companion_open(z, p, pfile, tdio::DT_I16, "int16_t", "flow direction grid does not match")) return rc;
+  const double dxA = fabs(z.dxc[z.ny / 2]), dyA = fabs(z.dyc[z.ny / 2]);
+  int niter = 0;
+  if (int rc = td_slopeavedown_niter(dn, dxA, dyA, &niter)) return rc;
+  if (td::mgpu_world() > 1 && z.ny >= td::mgpu_world()) {
+    td::MgpuSibJob J;
+    J.tool = td::MgpuSibJob::SLOPEAVEDOWN; J.dirfile = pfile; J.in[0] = felfile; J.dn = dn; J.niter = niter;
+    return sibling_multi_gpu(J, p, {{0, slpdfile, tdio::DT_F32, (double)-3.4028234663852886e38f}}, t0, "SlopeAveDown");
+  }
+  Warmup warm;
+  std::vector<float> fel;
+  std::vector<int16_t> dir;
+  if (int rc = z.read(&fel, tdio::DT_F32)) return rc;
+  if (int rc = p.read(&dir, tdio::DT_I16)) return rc;
+  warm.join();
+  const double t1 = now();
+  std::vector<float> sd((size_t)z.nx * z.ny);
+  if (int rc = td_slopeavedown_host(fel.data(), dir.data(), sd.data(), z.nx, z.ny, (float)z.r.nodata(), (int16_t)p.r.nodata(), z.dxc.data(), z.dyc.data(),
+                                    dxA, dyA, dn)) {
+    printf("SlopeAveDown device error: %s\n", td_last_error());
+    return rc;
+  }
+  const double t2 = now();
+  if (int rc = write_like(slpdfile, p, tdio::DT_F32, (double)-3.4028234663852886e38f, sd)) return rc;
+  const double t3 = now();
+  printf("Processors: 1\nRead time: %f\nCompute time: %f\nWrite time: %f\nTotal time: %f\n", t1 - t0, t2 - t1, t3 - t2, t3 - t0);
+  printf("Device compute time: %f\n", td_last_compute_seconds());
+  return TD_OK;
+} catch (const std::exception& e) {
+  td::set_error(std::string("exception: ") + e.what());
+  return TD_ERR_IO;
+}
+
 }  // extern "C"

@@ -178,6 +178,22 @@ int td_lengtharea_host(const float* plen, const int32_t* ad8, int16_t* ss, int n
 int td_sloped(const char* pfile, const char* felfile, const char* slpdfile, double dn);
 int td_slopeavedown_host(const float* fel, const int16_t* p, float* slpd, int nx, int ny, float fel_nodata, int16_t p_nodata, const double* dxc,
                          const double* dyc, double dx, double dy, double dn);
+/* flowdircond: D8-conditioned elevations.  Every cell the D8 queue of p reaches gets the smallest conditioned elevation among the
+ * cells that drain into it, or its own z if that is smaller, so that elevations never rise downstream along p; the other cells keep
+ * their z.  A cell whose z is nodata keeps it and still drains.  File level = `int flowdircond(char* pfile, char* zfile, char*
+ * zfdcfile)` (src/flowdircond.cpp:56; TD_ERR_MISMATCH when z and p differ in size).  zfdc: float32, the nodata value and the
+ * georeference of z.  Bit-exact. */
+int td_flowdircond(const char* pfile, const char* zfile, const char* zfdcfile);
+int td_flowdircond_host(const int16_t* p, const float* z, float* zfdc, int nx, int ny, int16_t p_nodata, float z_nodata);
+/* retlimflow: D-infinity retention-limited runoff, qrl = max(0, sum of p * qrl of the contributors + wg - rc) in float.  A cell whose
+ * wg or rc is nodata gets nodata and passes nothing on, so every cell downstream of it stays nodata.  File level = `int
+ * retlimro(char* angfile, char* wgfile, char* rcfile, char* qrlfile)` (src/RetlimFlow.cpp:53; TD_ERR_MISMATCH when a grid differs
+ * in size from ang).  qrl: float32, nodata MISSINGFLOAT, the georeference of rc.  dxc / dyc: per-row cell sizes.  TD_ERR_ARG when
+ * the angle nodata value is one prop() reads as a flow direction (above about -pi/4): the reference would add its share times
+ * MISSINGFLOAT.  Bit-exact. */
+int td_retlimro(const char* angfile, const char* wgfile, const char* rcfile, const char* qrlfile);
+int td_retlimflow_host(const float* ang, const float* wg, const float* rc, float* qrl, int nx, int ny, float ang_nodata, float wg_nodata, float rc_nodata,
+                       const double* dxc, const double* dyc);
 
 /* aread8 + areadinf of one DEM in one call (no weights, no outlets), the host<->device copies overlapped with the kernels
  * on three streams: p in -> aread8 || ang in -> areadinf || ad8 out -> sca out.  Same results as the two calls above.
@@ -331,6 +347,16 @@ int td_area_sweep_run_dev(td_ctx*, const float* ang, const float* w, float* sca,
 int td_d8flowpathextremeup_deps_dev(td_ctx*, const int16_t* p, float* ssa, td_strip s, int16_t p_nodata, void* stream);
 int td_d8flowpathextremeup_sweep_run_dev(td_ctx*, const float* sa, float* ssa, td_strip s, int usemax, int contcheck, int* halo_out,
                                          void* stream);
+/* flowdircond: halo rows of p and of z (the deps call starts zfdc as a copy of the whole strip of z, halo rows included; the sweep
+ * reads a halo row's value only after an exchange or a peer delivery) and overwrites the cells it evaluates.                    */
+int td_flowdircond_deps_dev(td_ctx*, const int16_t* p, const float* z, float* zfdc, td_strip s, int16_t p_nodata, void* stream);
+int td_flowdircond_sweep_run_dev(td_ctx*, const float* z, float* zfdc, td_strip s, float z_nodata, int* halo_out, void* stream);
+/* retlimflow: halo rows of ang (wg, rc: owned rows only).  qrl starts as MISSINGFLOAT.  The deps call reads dxc / dyc back to the
+ * host to check the angle nodata value (it synchronises the stream) and blocks the cells whose wg or rc is nodata.              */
+int td_retlimflow_deps_dev(td_ctx*, const float* ang, const float* wg, const float* rc, float* qrl, td_strip s, float ang_nodata,
+                           float wg_nodata, float rc_nodata, const double* dxc, const double* dyc, void* stream);
+int td_retlimflow_sweep_run_dev(td_ctx*, const float* ang, const float* wg, const float* rc, float* qrl, td_strip s, float wg_nodata,
+                                float rc_nodata, const double* dxc, int* halo_out, void* stream);
 /* dinfdecayaccum: halo rows of ang and dm (w: owned rows only, NULL = no weights).  dsca starts as MISSINGFLOAT.                */
 int td_dinfdecayaccum_deps_dev(td_ctx*, const float* ang, float* dsca, td_strip s, float ang_nodata, const double* dxc,
                                const double* dyc, void* stream);

@@ -73,6 +73,14 @@ SIGNATURES = {
     "td_slopeavedown_init_dev": (_I, [_P, _P, _P, _P, _P, _P, _P, Strip, C.c_int16, _F, _P]),
     "td_slopeavedown_pass_dev": (_I, [_P, _P, _P, _P, _P, _P, Strip, _P, _D, _P, _P]),
     "td_slopeavedown_niter": (_I, [_D, _D, _D, _P]),
+    "td_flowdircond": (_I, [_S, _S, _S]),
+    "td_flowdircond_host": (_I, [_P, _P, _P, _I, _I, C.c_int16, _F]),
+    "td_flowdircond_deps_dev": (_I, [_P, _P, _P, _P, Strip, C.c_int16, _P]),
+    "td_flowdircond_sweep_run_dev": (_I, [_P, _P, _P, Strip, _F, _P, _P]),
+    "td_retlimro": (_I, [_S, _S, _S, _S]),
+    "td_retlimflow_host": (_I, [_P, _P, _P, _P, _I, _I, _F, _F, _F, _P, _P]),
+    "td_retlimflow_deps_dev": (_I, [_P, _P, _P, _P, _P, Strip, _F, _F, _F, _P, _P, _P]),
+    "td_retlimflow_sweep_run_dev": (_I, [_P, _P, _P, _P, _P, Strip, _F, _F, _P, _P, _P]),
     "td_nameadd": (_I, [_S, _S, _S]),
     "td_raster_info": (_I, [_S] + [_P] * 9),
     "td_raster_read": (_I, [_S, _I, _P, _I, _I]),

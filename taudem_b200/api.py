@@ -322,6 +322,40 @@ def slopeavedown_grid(fel, p, dn=50.0, dx=30.0, dy=30.0, nodata=float(FEL_NODATA
     return slpd
 
 
+def flowdircond_grid(p, z, p_nodata=int(MISSINGSHORT), nodata=-9999.0):
+    """D8-conditioned elevations (td_flowdircond_host; src/flowdircond.cpp:143-194): every cell the aread8 queue of `p` reaches gets
+    the smallest conditioned elevation among the cells that drain into it, or its own z if that is smaller, so that elevations never
+    rise downstream along `p`; every other cell keeps its z.  A cell whose z is nodata (within 1e-5 of `nodata`) keeps it.  float32,
+    the nodata value of z."""
+    p = _grid(p, np.int16)
+    z = _grid(z, np.float32)
+    ny, nx = z.shape
+    if p.shape != z.shape:
+        raise ValueError("flowdircond_grid: p and z differ in shape")
+    zfdc = np.empty((ny, nx), np.float32)
+    check(lib().td_flowdircond_host(_ptr(p), _ptr(z), _ptr(zfdc), nx, ny, int(p_nodata), np.float32(nodata)))
+    return zfdc
+
+
+def retlimflow_grid(ang, wg, rc, dx=30.0, dy=30.0, ang_nodata=float(MISSINGFLOAT), wg_nodata=-9999.0, rc_nodata=-9999.0, dxc=None, dyc=None):
+    """D-infinity retention-limited runoff (td_retlimflow_host; src/RetlimFlow.cpp:147-200): qrl = max(0, sum of p * qrl of the
+    contributors + wg - rc) in float.  A cell whose wg or rc is nodata gets nodata and passes nothing on.  float32, nodata
+    MISSINGFLOAT.  dxc / dyc: per-row cell sizes (default dx / dy on every row).  An angle nodata value that prop() reads as a
+    direction raises TaudemError (code 1)."""
+    ang = _grid(ang, np.float32)
+    wg = _grid(wg, np.float32)
+    rc = _grid(rc, np.float32)
+    ny, nx = ang.shape
+    if wg.shape != ang.shape or rc.shape != ang.shape:
+        raise ValueError("retlimflow_grid: ang, wg and rc differ in shape")
+    dxc = _rows(dx if dxc is None else dxc, ny)
+    dyc = _rows(dy if dyc is None else dyc, ny)
+    qrl = np.empty((ny, nx), np.float32)
+    check(lib().td_retlimflow_host(_ptr(ang), _ptr(wg), _ptr(rc), _ptr(qrl), nx, ny, np.float32(ang_nodata), np.float32(wg_nodata), np.float32(rc_nodata),
+                                   _ptr(dxc), _ptr(dyc)))
+    return qrl
+
+
 def contributing_areas_grid(p, ang, p_nodata=int(MISSINGSHORT), ang_nodata=float(MISSINGFLOAT), dx=30.0, dy=30.0, contcheck=True, out_ad8=None, out_sca=None):
     """aread8 + areadinf of one DEM in one call, copies overlapped with the kernels (td_contributing_areas_host)."""
     p = _grid(p, np.int16); ang = _grid(ang, np.float32)

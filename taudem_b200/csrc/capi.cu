@@ -353,6 +353,68 @@ int td_d8flowpathextremeup_sweep_run_dev(td_ctx* ctx, const float* sa, float* ss
   if (int rc = check_strip(s)) return rc;
   return td::wsweep_run(ctx, false, ssa, sa, nullptr, Strip(s), 0.f, 1, contcheck, nullptr, nullptr, halo_out, (cudaStream_t)stream, usemax ? 1 : 2);
 }
+// flowdircond: the aread8 dependency state of p (the reference's queue is initNeighborD8up's, src/flowdircond.cpp:138), the output
+// starting as a copy of z (src/flowdircond.cpp:154-172 lowers z in place; cells the queue never reaches keep their z)
+int td_flowdircond_deps_dev(td_ctx* ctx, const int16_t* p, const float* z, float* zfdc, td_strip s, int16_t p_nodata, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  if (!p || !z || !zfdc) { td::set_error("td_flowdircond_deps_dev: bad arguments"); return TD_ERR_ARG; }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (int rc = ensure_dep_state(ctx, Strip(s), st)) return rc;
+  ctx->sweep_dinf = 0;
+  TD_CUDA(td::launch_deps_d8(p, ctx->node.as<unsigned short>(), ctx->cnt.as<unsigned char>(), zfdc, Strip(s), p_nodata, st));
+  TD_CUDA(cudaMemcpyAsync(zfdc, z, sizeof(float) * (size_t)Strip(s).cells(), cudaMemcpyDeviceToDevice, st));
+  return TD_OK;
+}
+int td_flowdircond_sweep_run_dev(td_ctx* ctx, const float* z, float* zfdc, td_strip s, float z_nodata, int* halo_out, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  return td::wsweep_run(ctx, false, zfdc, z, nullptr, Strip(s), z_nodata, 1, 0, nullptr, nullptr, halo_out, (cudaStream_t)stream, 11);
+}
+// retlimflow's gather reads a contributor's share with prop() without testing its angle for nodata (src/RetlimFlow.cpp:155-163):
+// a nodata value that prop() reads as a direction would add p * MISSINGFLOAT.  Such a value is refused, decided with prop() itself
+// (src/commonLib.cpp:76-91) on the cell sizes of every row a contributor can lie in (the strip's rows and its neighbours' edge rows).
+static double prop_host(float a, int k, double dx1, double dy1) {
+  double aref[10] = {-atan2(dy1, dx1), 0., 0., 0.5 * TD_PI, 0., TD_PI, 0., 1.5 * TD_PI, 0., 2. * TD_PI};
+  aref[2] = -aref[0]; aref[4] = TD_PI - aref[2]; aref[6] = TD_PI + aref[2]; aref[8] = 2. * TD_PI - aref[2];
+  double p = 0.;
+  if (k == 1 && a > TD_PI) a = (float)(a - 2.0 * TD_PI);
+  if (a > aref[k - 1] && a < aref[k + 1]) p = a > aref[k] ? (aref[k + 1] - a) / (aref[k + 1] - aref[k]) : (a - aref[k - 1]) / (aref[k] - aref[k - 1]);
+  return p < 1e-5 ? -1. : p;
+}
+static int check_ang_nodata(td_ctx* ctx, const td_strip& s, float ang_nodata, const double* dxc, const double* dyc) {
+  std::vector<double> dx((size_t)s.ny + 2), dy((size_t)s.ny + 2);
+  TD_CUDA(cudaMemcpy(dx.data(), dxc, sizeof(double) * s.ny, cudaMemcpyDeviceToHost));
+  TD_CUDA(cudaMemcpy(dy.data(), dyc, sizeof(double) * s.ny, cudaMemcpyDeviceToHost));
+  int n = s.ny;
+  for (int i = 0; i < 2; ++i)
+    if (ctx->halo_dx[i] > 0. && ctx->halo_dy[i] > 0.) { dx[n] = ctx->halo_dx[i]; dy[n] = ctx->halo_dy[i]; ++n; }
+  for (int r = 0; r < n; ++r) {
+    if (r > 0 && dx[r] == dx[r - 1] && dy[r] == dy[r - 1]) continue;
+    for (int k = 1; k <= 8; ++k)
+      if (prop_host(ang_nodata, k, dx[r], dy[r]) > 0.) {
+        td::set_error("retlimflow: the angle nodata value " + std::to_string(ang_nodata) + " is a flow direction to prop(); the reference would add its "
+                      "share times MISSINGFLOAT (use a nodata value below -pi/4, e.g. -FLT_MAX)");
+        return TD_ERR_ARG;
+      }
+  }
+  return TD_OK;
+}
+// retlimflow: the areadinf dependency state of ang (initNeighborDinfup, src/RetlimFlow.cpp:128), qrl starting as MISSINGFLOAT,
+// then the cells whose wg or rc is nodata blocked (launch_block_cells)
+int td_retlimflow_deps_dev(td_ctx* ctx, const float* ang, const float* wg, const float* rc, float* qrl, td_strip s, float ang_nodata, float wg_nodata,
+                           float rc_nodata, const double* dxc, const double* dyc, void* stream) {
+  if (int rc_ = check_strip(s)) return rc_;
+  if (!ang || !wg || !rc || !qrl || !dxc || !dyc) { td::set_error("td_retlimflow_deps_dev: bad arguments"); return TD_ERR_ARG; }
+  if (int e = check_ang_nodata(ctx, s, ang_nodata, dxc, dyc)) return e;
+  if (int e = area_deps(ctx, ang, qrl, s, ang_nodata, dxc, dyc, false, stream, TD_MISSINGFLOAT)) return e;
+  TD_CUDA(td::launch_block_cells(ctx->node.as<unsigned short>(), wg, wg_nodata, rc, rc_nodata, Strip(s), (cudaStream_t)stream));
+  return TD_OK;
+}
+int td_retlimflow_sweep_run_dev(td_ctx* ctx, const float* ang, const float* wg, const float* rc, float* qrl, td_strip s, float wg_nodata, float rc_nodata,
+                                const double* dxc, int* halo_out, void* stream) {
+  if (int e = check_strip(s)) return e;
+  return td::wsweep_run(ctx, true, qrl, wg, ang, Strip(s), wg_nodata, 1, 0, ctx->theta.as<double>(), dxc, halo_out, (cudaStream_t)stream, 12, rc,
+                        rc_nodata);
+}
 int td_dinfdecayaccum_deps_dev(td_ctx* ctx, const float* ang, float* dsca, td_strip s, float ang_nodata, const double* dxc, const double* dyc, void* stream) {
   return area_deps(ctx, ang, dsca, s, ang_nodata, dxc, dyc, false, stream, TD_MISSINGFLOAT);
 }
@@ -598,6 +660,54 @@ int td_d8flowpathextremeup_host(const int16_t* p, const float* sa, float* ssa, i
   if (int rc = td_d8flowpathextremeup_sweep_run_dev(ctx, d_sa, d_a, s, usemax, contcheck, ctx->halo.as<int>(), st)) return rc;
   td::set_compute_seconds(t.stop(st));
   TD_CUDA(d2h(ssa, d_a, s, st));
+  TD_CUDA(cudaStreamSynchronize(st));
+  return TD_OK;
+}
+
+// ---- flowdircond (src/flowdircond.cpp:56-194): the D8 dependency stencil and sweep of p with the conditioning algebra (11).
+int td_flowdircond_host(const int16_t* p, const float* z, float* zfdc, int nx, int ny, int16_t p_nodata, float z_nodata) {
+  if (int rc = need_device()) return rc;
+  if (!p || !z || !zfdc || nx <= 0 || ny <= 0) { td::set_error("td_flowdircond_host: bad arguments"); return TD_ERR_ARG; }
+  td_ctx* ctx = default_ctx();
+  const td_strip s = host_strip(nx, ny);
+  const size_t n = (size_t)Strip(s).cells();
+  cudaStream_t st = 0;
+  TD_CUDA(ctx->io[0].ensure(n * 2)); TD_CUDA(ctx->io[1].ensure(n * 4)); TD_CUDA(ctx->io[2].ensure(n * 4));
+  int16_t* d_p = ctx->io[0].as<int16_t>(); float* d_a = ctx->io[1].as<float>(); float* d_z = ctx->io[2].as<float>();
+  TD_CUDA(h2d(d_p, p, s, st));
+  TD_CUDA(h2d(d_z, z, s, st));
+  Timer t; t.start(st);
+  if (int rc = td_flowdircond_deps_dev(ctx, d_p, d_z, d_a, s, p_nodata, st)) return rc;
+  if (int rc = td_sweep_begin_dev(ctx, s, st)) return rc;
+  if (int rc = td_flowdircond_sweep_run_dev(ctx, d_z, d_a, s, z_nodata, ctx->halo.as<int>(), st)) return rc;
+  td::set_compute_seconds(t.stop(st));
+  TD_CUDA(d2h(zfdc, d_a, s, st));
+  TD_CUDA(cudaStreamSynchronize(st));
+  return TD_OK;
+}
+
+// ---- retlimflow (src/RetlimFlow.cpp:53-240): the D-infinity dependency stencil and sweep with the retention-limited algebra (12).
+int td_retlimflow_host(const float* ang, const float* wg, const float* rc, float* qrl, int nx, int ny, float ang_nodata, float wg_nodata, float rc_nodata,
+                       const double* dxc, const double* dyc) {
+  if (int e = need_device()) return e;
+  if (!ang || !wg || !rc || !qrl || !dxc || !dyc || nx <= 0 || ny <= 0) { td::set_error("td_retlimflow_host: bad arguments"); return TD_ERR_ARG; }
+  td_ctx* ctx = default_ctx();
+  const td_strip s = host_strip(nx, ny);
+  const size_t n = (size_t)Strip(s).cells();
+  cudaStream_t st = 0;
+  TD_CUDA(ctx->io[0].ensure(n * 4)); TD_CUDA(ctx->io[1].ensure(n * 4)); TD_CUDA(ctx->io[2].ensure(n * 4)); TD_CUDA(ctx->io[3].ensure(n * 4));
+  float* d_ang = ctx->io[0].as<float>(); float* d_a = ctx->io[1].as<float>(); float* d_wg = ctx->io[2].as<float>(); float* d_rc = ctx->io[3].as<float>();
+  const double *d_dx, *d_dy;
+  if (int e = upload_rows(ctx, dxc, dyc, ny, &d_dx, &d_dy, st)) return e;
+  TD_CUDA(h2d(d_ang, ang, s, st));
+  TD_CUDA(h2d(d_wg, wg, s, st));
+  TD_CUDA(h2d(d_rc, rc, s, st));
+  Timer t; t.start(st);
+  if (int e = td_retlimflow_deps_dev(ctx, d_ang, d_wg, d_rc, d_a, s, ang_nodata, wg_nodata, rc_nodata, d_dx, d_dy, st)) return e;
+  if (int e = td_sweep_begin_dev(ctx, s, st)) return e;
+  if (int e = td_retlimflow_sweep_run_dev(ctx, d_ang, d_wg, d_rc, d_a, s, wg_nodata, rc_nodata, d_dx, ctx->halo.as<int>(), st)) return e;
+  td::set_compute_seconds(t.stop(st));
+  TD_CUDA(d2h(qrl, d_a, s, st));
   TD_CUDA(cudaStreamSynchronize(st));
   return TD_OK;
 }

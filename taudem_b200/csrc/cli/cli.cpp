@@ -1,5 +1,5 @@
 // Command line front ends: pitremove, d8flowdir, dinfflowdir, aread8, areadinf (+ the point-wise consumers threshold, twi, slopearea, slopearearatio,
-// the sibling sweep tools, the stream definitions peukerdouglas and lengtharea, and slopeavedown).
+// the sibling sweep tools, the stream definitions peukerdouglas and lengtharea, slopeavedown, flowdircond and retlimflow).
 // Same flags, same two invocation styles and the same "print usage and exit(0)" error
 // behaviour as the reference mains (src/PitRemovemn.cpp:48-172, src/D8FlowDirmn.cpp:49-146,
 // src/DinfFlowDirmn.cpp:54-147, src/aread8mn.cpp:49-193, src/areadinfmn.cpp:49-178);
@@ -517,6 +517,54 @@ int main(int argc, char** argv) {
   if (argc == 2) { td_nameadd(fel, argv[1], "fel"); td_nameadd(p, argv[1], "p"); td_nameadd(slpd, argv[1], "slpd"); }
   int err = td_sloped(p, fel, slpd, dn);
   if (err != 0) printf("sloped error %d\n", err);
+  return done();
+}
+#elif defined(TOOL_flowdircond)
+// src/flowdirconditionmn.cpp:55-128 (the reference's usage text, without a "Simple Usage" line, and its error line as printed)
+static void usage(const char* prog) {
+  printf("Use with specific file names:\n %s -p <pfile>\n", prog);
+  printf("-z <zfile> -zfdc <zfdcfile> \n");
+  printf("<pfile> is the name of the input D8 flow direction raster file.\n");
+  printf("<zfile> is the name of the input elevation raster file.\n");
+  printf("<zfdcfile> is the name of the output conditioned elevation raster file.\n");
+  exit(0);
+}
+int main(int argc, char** argv) {
+  static char p[MAXLN], z[MAXLN], zfdc[MAXLN];
+  Opt opts[] = {{"-z", 0, z, NULL, 0}, {"-p", 0, p, NULL, 0}, {"-zfdc", 0, zfdc, NULL, 0}};
+  parse(argc, argv, opts, 3);
+  if (argc == 2) { td_nameadd(z, argv[1], "z"); td_nameadd(p, argv[1], "p"); td_nameadd(zfdc, argv[1], "zfdc"); }
+  int err = td_flowdircond(p, z, zfdc);
+  if (err != 0) printf("flowdiircond error %d\n", err);
+  return done();
+}
+#elif defined(TOOL_retlimflow)
+// src/RetLimFlowmn.cpp:51-146 (the reference's usage text; its error line always shows 1: `err=retlimro(...) != 0` assigns the
+// comparison)
+static void usage(const char* prog) {
+  printf("Simple Usage:\n %s <basefilename>\n", prog);
+  printf("Usage with specific file names:\n %s -ang <angfile>", prog);
+  printf("-rc <rcfile> -wg <wgfile> -qrl <qrlfile>\n");
+  printf("<basefilename> is the name of the raw digital elevation model\n");
+  printf("<angfile> is the D-infinity flow direction input file.\n");
+  printf("<rcfile> retention capacity file.\n");
+  printf("<wgfile> is the input weight at each grid cell.\n");
+  printf("<qrlfile> is retention limited runoff that is output.\n");
+  printf("With simple use the following are appended to the file names\n");
+  printf("before the files are opened:\n");
+  printf("ang    D-infinity flow direction input file\n");
+  printf("rc    retention capacity (input)\n");
+  printf("wg     weight grid (input)\n");
+  printf("qrl   retention limited runoff (output)\n");
+  exit(0);
+}
+int main(int argc, char** argv) {
+  static char ang[MAXLN], wg[MAXLN], rc[MAXLN], qrl[MAXLN];
+  Opt opts[] = {{"-ang", 0, ang, NULL, 0}, {"-wg", 0, wg, NULL, 0}, {"-rc", 0, rc, NULL, 0}, {"-qrl", 0, qrl, NULL, 0}};
+  parse(argc, argv, opts, 4);
+  if (argc == 2) { td_nameadd(ang, argv[1], "ang"); td_nameadd(rc, argv[1], "rc"); td_nameadd(qrl, argv[1], "qrl"); td_nameadd(wg, argv[1], "wg"); }
+  int err = td_retlimro(ang, wg, rc, qrl) != 0;
+  if (err) printf("RetlimFlow error %d\n", err);
   return done();
 }
 #else

@@ -49,7 +49,7 @@ struct td_ctx {
   td::PropRow prop;                      // prop() table of the strip whose theta table is loaded (uniform = 0: rows differ)
   double dx0 = 0.;                       // cell size of the strip's rows when they all have the same (prop.uniform)
   double halo_dx[2] = {0., 0.}, halo_dy[2] = {0., 0.};   // cell sizes of the neighbour strips' edge rows (row above / below; <= 0: not set, the strip's own edge rows stand in)
-  static constexpr int SWEEP_KERNELS = 14;   // instantiations of the warp-per-tile sweep kernel (the table SWEEPS in sweep_warp.cu)
+  static constexpr int SWEEP_KERNELS = 16;   // instantiations of the warp-per-tile sweep kernel (the table SWEEPS in sweep_warp.cu)
   int wgrid[SWEEP_KERNELS] = {0};         // persistent grid of each of them on this context's device
   static constexpr int NCTR = 40;        // device counters: [24..32] the contributing-area sweep's statistics (sweep_warp.cu WArgs::stat),
                                          // [36] slopeavedown's changed flag (capi.cu)

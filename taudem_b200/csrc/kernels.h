@@ -17,7 +17,9 @@ cudaError_t launch_deps_d8(const short* p, unsigned short* node, unsigned char* 
 cudaError_t launch_halo_codes_d8(const short* p, unsigned short* node, const Strip& s, short nodata, cudaStream_t st);   // gridnet on row strips
 cudaError_t launch_deps_dinf(const float* ang, unsigned short* node, unsigned char* cnt, float* area, const Strip& s,
                              float nodata, const double* theta, cudaStream_t st, float area_init = -1.0f);
-cudaError_t zero_words(void* p, size_t bytes, cudaStream_t st);     // a multiple of 4 bytes, zeroed by a kernel (never by a copy engine)
+cudaError_t zero_words(void* p, size_t bytes, cudaStream_t st);
+// retlimflow: cells of the owned rows whose wg or rc is nodata lose their receivers in the node words (sweep_warp.cu)
+cudaError_t launch_block_cells(unsigned short* node, const float* wg, float wg_nodata, const float* rc, float rc_nodata, const Strip& s, cudaStream_t st);     // a multiple of 4 bytes, zeroed by a kernel (never by a copy engine)
 int wsweep_begin(td_ctx* ctx, const Strip& s, cudaStream_t st);
 int wsweep_apply_halo(td_ctx* ctx, const Strip& s, const int* dec_top, const int* dec_bot, cudaStream_t st);
 // the extra grids of the concentration- and transport-limited accumulations (algebras 7-9 of the D-infinity sweep, sweep_warp.cu)

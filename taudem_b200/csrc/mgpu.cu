@@ -1,6 +1,6 @@
 // Multi-GPU contributing area behind the executables: `TAUDEM_B200_GPUS=N aread8 ...` / `areadinf ...`, and the same for the five
 // sibling sweep tools (d8flowpathextremeup, gridnet, dinfdecayaccum, dinfconclimaccum, dinftranslimaccum: sibling_worker), and
-// slopeavedown, whose passes follow its D8 sweep there.
+// slopeavedown, whose passes follow its D8 sweep there, flowdircond and retlimflow.
 //
 // reference: the callers' contract is `mpiexec -n N aread8` (src/aread8.cpp:57,100: MPI_Init, one row strip per rank,
 // src/linearpart.h:160-200 the partition, src/aread8.cpp:280-304 the border exchange + ringTerm loop).  Here the
@@ -273,7 +273,7 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
   cudaStream_t st;
   MG_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
 
-  const bool dinf = J.tool >= MgpuSibJob::DECAY && J.tool <= MgpuSibJob::TRANSLIM;
+  const bool dinf = (J.tool >= MgpuSibJob::DECAY && J.tool <= MgpuSibJob::TRANSLIM) || J.tool == MgpuSibJob::RETLIMFLOW;
   tdio::Raster in;
   std::string err;
   if (!in.open(J.dirfile, &err)) throw Fail{"open " + std::string(J.dirfile) + ": " + err};
@@ -288,8 +288,9 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
   MG_CUDA(cudaMalloc(&d_dir, cells * tdio::dtype_bytes(dt)));
   load_strip(in, dt, d_dir, nx, s.pitch, row0, ny, total_ny, st);
   // the further inputs, each with its halo rows (MgpuSibJob::in)
-  static const tdio::DType in_type[6][3] = {{tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}, {tdio::DT_I32, tdio::DT_F32, tdio::DT_F32},
+  static const tdio::DType in_type[8][3] = {{tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}, {tdio::DT_I32, tdio::DT_F32, tdio::DT_F32},
                                             {tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}, {tdio::DT_F32, tdio::DT_F32, tdio::DT_I16},
+                                            {tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}, {tdio::DT_F32, tdio::DT_F32, tdio::DT_F32},
                                             {tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}, {tdio::DT_F32, tdio::DT_F32, tdio::DT_F32}};
   tdio::Raster rin[3];
   void* d_in[3] = {nullptr, nullptr, nullptr};
@@ -382,6 +383,14 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
       MG_TD(td_dinfconclimaccum_deps_dev(ctx, ang, d_val, s, a_nd, d_dx, d_dx + ny, st));
       one_sweep([&]() { MG_TD(td_dinfconclimaccum_sweep_run_dev(ctx, ang, f0, f1, (const int16_t*)d_in[2], d_val, s, nd[0], nd[1], J.csol, J.contcheck, d_dx,
                                                                 d_halo, st)); }, nullptr);
+      break;
+    case MgpuSibJob::FLOWDIRCOND:
+      MG_TD(td_flowdircond_deps_dev(ctx, (const int16_t*)d_dir, f0, d_val, s, p_nd, st));
+      one_sweep([&]() { MG_TD(td_flowdircond_sweep_run_dev(ctx, f0, d_val, s, nd[0], d_halo, st)); }, nullptr);
+      break;
+    case MgpuSibJob::RETLIMFLOW:
+      MG_TD(td_retlimflow_deps_dev(ctx, ang, f0, f1, d_val, s, a_nd, nd[0], nd[1], d_dx, d_dx + ny, st));
+      one_sweep([&]() { MG_TD(td_retlimflow_sweep_run_dev(ctx, ang, f0, f1, d_val, s, nd[0], nd[1], d_dx, d_halo, st)); }, nullptr);
       break;
     case MgpuSibJob::SLOPEAVEDOWN: {
       // the D8 sweep marks the cells the reference's queue processes; then the passes, each followed by the exchange of the state's
@@ -672,7 +681,7 @@ int mgpu_area(const MgpuJob& J, int world, double* compute_seconds, int* rounds)
 int mgpu_sibling(const MgpuSibJob& J, int world, double* compute_seconds, int* rounds) {
   if (world < 2 || world > MAXR) { set_error("mgpu_sibling: between 2 and 64 ranks"); return TD_ERR_ARG; }
   if (J.ny < world) { set_error("mgpu_sibling: fewer rows than ranks"); return TD_ERR_ARG; }
-  if (J.tool < MgpuSibJob::EXTREMEUP || J.tool > MgpuSibJob::SLOPEAVEDOWN || !J.out[0]) { set_error("mgpu_sibling: bad job"); return TD_ERR_ARG; }
+  if (J.tool < MgpuSibJob::EXTREMEUP || J.tool > MgpuSibJob::RETLIMFLOW || !J.out[0]) { set_error("mgpu_sibling: bad job"); return TD_ERR_ARG; }
   const int pitch = td_pitch_for(J.nx);
   return run_ranks("mgpu_sibling", world, RoundBuf::bytes(pitch) * (size_t)world,
                    [&](Shared* S, char* extra, int r) { sibling_worker(J, S, extra, r, world); }, compute_seconds, rounds, nullptr);

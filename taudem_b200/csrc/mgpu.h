@@ -31,8 +31,10 @@ struct MgpuFlowJob {
 //   CONCLIM    dinfconclimaccum     in: dm, q, dg (int16)  out: ctpt
 //   TRANSLIM   dinftranslimaccum    in: tsup, tc, cs       out: tla, tdep, ctpt (with cs)
 //   SLOPEAVEDOWN  slopeavedown      in: fel                out: slpd (the D8 sweep of p, then niter passes at dn)
+//   FLOWDIRCOND   flowdircond       in: z                  out: zfdc
+//   RETLIMFLOW    retlimflow        in: wg, rc             out: qrl
 struct MgpuSibJob {
-  enum { EXTREMEUP = 0, GRIDNET, DECAY, CONCLIM, TRANSLIM, SLOPEAVEDOWN };
+  enum { EXTREMEUP = 0, GRIDNET, DECAY, CONCLIM, TRANSLIM, SLOPEAVEDOWN, FLOWDIRCOND, RETLIMFLOW };
   int tool = EXTREMEUP;
   const char* dirfile = nullptr;              // p (D8 tools) or ang
   const char* in[3] = {nullptr, nullptr, nullptr};

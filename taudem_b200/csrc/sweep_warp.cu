@@ -389,6 +389,23 @@ __global__ void k_wsched_init(int* state, int* tq, int ntiles, unsigned long lon
   }
 }
 
+// The NaN that x86 SSE arithmetic gives (the reference's; ALG 12, where a NaN wg travels): a NaN result carries the first NaN
+// operand, quieted, and an invalid operation on numbers (inf - inf, 0 * inf) gives the default NaN 0xffc00000.  The GPU's own NaN
+// result is 0x7fffffff.
+__device__ __forceinline__ float quiet_bits(float a, unsigned set) {
+  unsigned u;
+  memcpy(&u, &a, 4);
+  u |= set;
+  memcpy(&a, &u, 4);
+  return a;
+}
+__device__ __forceinline__ float x86_nan(float r, float a, float b) {
+  if (r == r) return r;
+  if (a != a) return quiet_bits(a, 0x00400000u);
+  if (b != b) return quiet_bits(b, 0x00400000u);
+  return quiet_bits(0.f, 0xffc00000u);
+}
+
 // prop(angle, kk) through the full interval search (irregular cells, strips whose rows have different cell sizes)
 __device__ __noinline__ double wshare_full(float ang, double t, int kk) {
   const Outflow o = dinf_outflow(ang, t);
@@ -417,7 +434,12 @@ __device__ __forceinline__ unsigned zero_nibble(unsigned w) {
 // `w` = supply, `dm` = transport capacity, the value that travels is the transport out of the cell; deposition goes straight to
 // x.out2; with a concentration (9) a second value travels: it lives in global memory (x.out3) — written before the receivers'
 // counts are touched, read past the L1 — because a worker's shared memory holds one value per cell).
-// Results of ALG 1-3 and 7-9 use MISSINGFLOAT as nodata, the others -1.
+// D8 with `w` = the raw elevation: 11 = flowdircond (src/flowdircond.cpp:143-194; the output starts as a copy of `w` and keeps it where
+// the sweep never evaluates; no contamination, the caller passes contcheck = 0).
+// D-infinity with `w` = the weight wg and `dm` = the retention capacity rc, one chain per lane throughout: 12 = retlimflow
+// (src/RetlimFlow.cpp:147-200: qrl = max(0, sum of (float)p * qrl of the contributors + wg - rc) in float; a cell whose wg or rc is
+// nodata gets nodata and, through launch_block_cells, decrements no receiver).
+// Results of ALG 1-3, 7-9 and 12 use MISSINGFLOAT as nodata, ALG 11 the nodata of `w`, the others -1.
 // gridnet's cell evaluation (src/gridnet.cpp:383-420): contributors = the neighbours that drain into the cell (mask bits) with a
 // direction > 0 and inside the mask; all arithmetic in float like the reference's float dist table and float partitions.
 template <int ALG, typename Mem>
@@ -447,6 +469,21 @@ __device__ __forceinline__ float gridnet_eval(const WArgs& a, const Mem& M, int 
 struct Eval { float val; bool con; };
 template <bool USEW, int ALG, typename Mem>
 __device__ __forceinline__ Eval d8_gather(const WArgs& a, const Mem& M, int ri, unsigned msk, int r, int c, float wv, float NOD, bool con) {
+  if (ALG == 11) {
+    // flowdircond (src/flowdircond.cpp:154-172): `w` = the raw elevation z, the travelling value = the conditioned z.  A cell whose z
+    // is nodata keeps it; otherwise the smallest conditioned z of its contributors that is not nodata, by the reference's strict
+    // test in increasing k (a NaN never replaces a value, -0 never replaces +0).  (The reference also skips contributors with code
+    // 0; a cell that counts one — the cell south-east of a code 0 — is never ready, so the test would be dead here.)
+    float val = wv;
+    if (nd_f(wv, a.w_nodata)) return {val, con};
+#pragma unroll
+    for (int k = 1; k <= 8; ++k)
+      if (msk & (1u << (k - 1))) {
+        const float zn = M.area[ri + drow(k) * RS + dcol(k)];
+        if (!nd_f(zn, a.w_nodata) && zn < val) val = zn;
+      }
+    return {val, con};
+  }
   if (ALG >= 4) return {gridnet_eval<ALG>(a, M, ri, msk, r, c), con};
   if (USEW) {
     float val = (ALG == 0 && nd_f(wv, a.w_nodata)) ? -1.0f : wv;
@@ -612,7 +649,7 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
         }
       }
       const unsigned act = __ballot_sync(FULL, cur >= 0);
-      if (ALG < 7 && act != 0u && (act & (act - 1u)) == 0u) {
+      if ((ALG < 7 || ALG == 11) && act != 0u && (act & (act - 1u)) == 0u) {
         // ---- one chain left (a river crossing the tile, the tail of every visit; the fork stack is empty, or idle lanes
         // would have taken from it): the WHOLE warp follows it together.  Nothing diverges and nothing is contended: the cell
         // is warp-uniform, lanes 0..7 evaluate one contributor link each (D-infinity), everybody folds the products in
@@ -750,6 +787,10 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
                                                                          : ldv(a.x.out3 + s.idx(rn, cc));
                 if (nd_f(cn, NOD)) con = true; else loadin = (float)((double)loadin + (p * (double)nt) * (double)cn);
               }
+            } else if (ALG == 12) {
+              // src/RetlimFlow.cpp:158-163: a float share times the contributor's qrl, summed in float
+              const float pf = (float)p;
+              if (pf > 0.f) { const float pq = x86_nan(pf * an, pf, an); val = x86_nan(val + pq, val, pq); }
             } else if (nd_f(an, NOD)) con = true; else val = (float)((double)val + p * (double)an);
           }
           if (ALG == 3) {}
@@ -785,6 +826,11 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
               if (ALG == 9) { stv(a.x.out3 + gc, bad ? NOD : cs); __threadfence_block(); }
               val = transout;
             }
+          } else if (ALG == 12) {
+            // src/RetlimFlow.cpp:151,165-166: (qrl + wg) - rc, clipped at 0 by `< 0` (a -0 and a NaN stay)
+            const float rcv = __ldg(a.dm + s.idx(r, c0 + lx));
+            if (nd_f(wv, a.w_nodata) || nd_f(rcv, a.dm_nodata)) val = NOD;
+            else { const float t = x86_nan(val + wv, val, wv); val = x86_nan(t - rcv, t, rcv); if (val < 0.f) val = 0.f; }
           }
           else if (USEW) val = val + wv;
           else val = (float)((double)val + own_area(a, r));
@@ -953,6 +999,20 @@ __global__ void __launch_bounds__(workers_per_cta<DINF>() * 32, 1) k_sweep_warp(
   }
 }
 
+// retlimflow (src/RetlimFlow.cpp:151,168-189): a cell whose wg or rc is nodata is evaluated (to nodata) but decrements no receiver,
+// so nothing downstream of it is ever evaluated.  Its node word loses its receivers — the receiver field and the second-receiver
+// bit 0x2000 — like an adopted outlet's (outlets.cu); its receivers keep counting it.  Owned rows only: the owner of a cell is
+// the only strip that delivers from it.
+__global__ void k_block_cells(unsigned short* __restrict__ node, const float* __restrict__ wg, float wg_nodata, const float* __restrict__ rc,
+                              float rc_nodata, Strip s) {
+  const long long n = (long long)s.ny * s.pitch;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long ci = s.pitch + i;
+    if ((int)(i % s.pitch) >= s.nx) continue;
+    if (nd_f(wg[ci], wg_nodata) || nd_f(rc[ci], rc_nodata)) node[ci] = (unsigned short)(node[ci] & ~0x2f00u);
+  }
+}
+
 // Applies the dependency decrements received from the neighbour strips (addBorders, src/linearpart.h:314-328 and
 // src/aread8.cpp:283-297): dec_top[c] arrivals for the cell (row 1, c), dec_bot[c] for (row ny, c).  A count that
 // reaches zero queues the cell's tile.
@@ -1033,9 +1093,18 @@ const SweepKernel SWEEPS[] = {
     sweep_kernel<true, true, 7>(NEED_W | NEED_DM | NEED_EXTRA | NEED_DG),
     sweep_kernel<true, true, 8>(NEED_W | NEED_DM | NEED_EXTRA | NEED_OUT2),
     sweep_kernel<true, true, 9>(NEED_W | NEED_DM | NEED_EXTRA | NEED_OUT2 | NEED_CIN | NEED_OUT3),
+    sweep_kernel<false, true, 11>(NEED_W),
+    sweep_kernel<true, true, 12>(NEED_W | NEED_DM),
 };
 static_assert(sizeof(SWEEPS) / sizeof(SWEEPS[0]) == td_ctx::SWEEP_KERNELS, "td_ctx::wgrid has one slot per sweep kernel");
 }  // namespace
+
+cudaError_t launch_block_cells(unsigned short* node, const float* wg, float wg_nodata, const float* rc, float rc_nodata, const Strip& s, cudaStream_t st) {
+  const size_t n = (size_t)s.ny * s.pitch;
+  k_block_cells<<<fill_grid(n), 256, 0, st>>>(node, wg, wg_nodata, rc, rc_nodata, s);
+  TD_LAUNCHED();
+  return cudaGetLastError();
+}
 
 // Queues every tile of the strip (start of a sweep).
 int wsweep_begin(td_ctx* ctx, const Strip& s, cudaStream_t st) {

@@ -984,4 +984,85 @@ int td_sloped(const char* pfile, const char* felfile, const char* slpdfile, doub
   return TD_ERR_IO;
 }
 
+// src/flowdircond.cpp:56-236: p (int16) and z (float) in, zfdc out (float32, the nodata value and the georeference of z: the reference
+// writes zIO.getNodata(), the double of z's header).
+// TAUDEM_B200_GPUS=N runs it on N row strips.
+int td_flowdircond(const char* pfile, const char* zfile, const char* zfdcfile) try {
+  printf("FlowDirCond version %s\n", td_version());
+  fflush(stdout);
+  const double t0 = now();
+  Input p;
+  if (int rc = p.open(pfile)) return rc;
+  nodata_msgs(p.r.nodata(), "int16_t", (int16_t)p.r.nodata());
+  Input z;
+  if (int rc = companion_open(p, z, zfile, tdio::DT_F32, "float", "elevation grid does not match")) return rc;
+  if (use_multi_gpu(p, 0)) {
+    td::MgpuSibJob J;
+    J.tool = td::MgpuSibJob::FLOWDIRCOND; J.dirfile = pfile; J.in[0] = zfile;
+    return sibling_multi_gpu(J, z, {{0, zfdcfile, tdio::DT_F32, z.r.nodata()}}, t0, "FlowDirCond");
+  }
+  Warmup warm;
+  std::vector<int16_t> dir;
+  std::vector<float> zv;
+  if (int rc = p.read(&dir, tdio::DT_I16)) return rc;
+  if (int rc = z.read(&zv, tdio::DT_F32)) return rc;
+  warm.join();
+  const double t1 = now();
+  std::vector<float> out((size_t)p.nx * p.ny);
+  if (int rc = td_flowdircond_host(dir.data(), zv.data(), out.data(), p.nx, p.ny, (int16_t)p.r.nodata(), (float)z.r.nodata())) {
+    printf("FlowDirCond device error: %s\n", td_last_error());
+    return rc;
+  }
+  const double t2 = now();
+  if (int rc = write_like(zfdcfile, z, tdio::DT_F32, z.r.nodata(), out)) return rc;
+  const double t3 = now();
+  printf("Processors: 1\nRead time: %f\nCompute time: %f\nWrite time: %f\nTotal time: %f\n", t1 - t0, t2 - t1, t3 - t2, t3 - t0);
+  printf("Device compute time: %f\n", td_last_compute_seconds());
+  return TD_OK;
+} catch (const std::exception& e) {
+  td::set_error(std::string("exception: ") + e.what());
+  return TD_ERR_IO;
+}
+
+// src/RetlimFlow.cpp:53-240: ang, wg and rc (float) in, qrl out (float32, nodata MISSINGFLOAT, the georeference of rc).  The shares use
+// ang's per-row cell sizes.  TAUDEM_B200_GPUS=N runs it on N row strips.
+int td_retlimro(const char* angfile, const char* wgfile, const char* rcfile, const char* qrlfile) try {
+  printf("Retention limited flow accumulation version %s\n", td_version());
+  fflush(stdout);
+  const double t0 = now();
+  Input a;
+  if (int rc = a.open(angfile)) return rc;
+  nodata_msgs(a.r.nodata(), "float", (float)a.r.nodata());
+  Input w, r;
+  if (int rc = companion_open(a, w, wgfile, tdio::DT_F32, "float", "weight grid does not match")) return rc;
+  if (int rc = companion_open(a, r, rcfile, tdio::DT_F32, "float", "retention capacity grid does not match")) return rc;
+  if (use_multi_gpu(a, 0)) {
+    td::MgpuSibJob J;
+    J.tool = td::MgpuSibJob::RETLIMFLOW; J.dirfile = angfile; J.in[0] = wgfile; J.in[1] = rcfile;
+    return sibling_multi_gpu(J, r, {{0, qrlfile, tdio::DT_F32, (double)-3.4028234663852886e38f}}, t0, "RetlimFlow");
+  }
+  Warmup warm;
+  std::vector<float> ang, wg, rcv;
+  if (int rc = a.read(&ang, tdio::DT_F32)) return rc;
+  if (int rc = w.read(&wg, tdio::DT_F32)) return rc;
+  if (int rc = r.read(&rcv, tdio::DT_F32)) return rc;
+  warm.join();
+  const double t1 = now();
+  std::vector<float> out((size_t)a.nx * a.ny);
+  if (int rc = td_retlimflow_host(ang.data(), wg.data(), rcv.data(), out.data(), a.nx, a.ny, (float)a.r.nodata(), (float)w.r.nodata(), (float)r.r.nodata(),
+                                  a.dxc.data(), a.dyc.data())) {
+    printf("RetlimFlow device error: %s\n", td_last_error());
+    return rc;
+  }
+  const double t2 = now();
+  if (int rc = write_like(qrlfile, r, tdio::DT_F32, (double)-3.4028234663852886e38f, out)) return rc;
+  const double t3 = now();
+  printf("Processors: 1\nRead time: %f\nCompute time: %f\nWrite time: %f\nTotal time: %f\n", t1 - t0, t2 - t1, t3 - t2, t3 - t0);
+  printf("Device compute time: %f\n", td_last_compute_seconds());
+  return TD_OK;
+} catch (const std::exception& e) {
+  td::set_error(std::string("exception: ") + e.what());
+  return TD_ERR_IO;
+}
+
 }  // extern "C"

@@ -3,15 +3,7 @@
 #include <stddef.h>
 
 namespace td {
-struct MgpuJob {
-  int dinf = 0;                 // 0 = aread8 (int16 directions), 1 = areadinf (float angles)
-  const char* dirfile = nullptr;
-  const char* wfile = nullptr;  // weight grid (usew)
-  int usew = 0, contcheck = 1;
-  int nx = 0, ny = 0;
-  float* out = nullptr;         // nx * ny floats in a mapping from mgpu_alloc_shared: every rank stores its rows
-};
-// the other three tools of the path on row strips: tool 0 = pitremove (out0 = fel), 1 = d8flowdir (out0 = p int16, out1 = sd8),
+// pitremove, the flow directions and peukerdouglas on row strips: tool 0 = pitremove (out0 = fel), 1 = d8flowdir (out0 = p int16, out1 = sd8),
 // 2 = dinfflowdir (out0 = ang, out1 = slp), 3 = peukerdouglas (out0 = ss int16); the rasters live in mappings from mgpu_alloc_shared
 struct MgpuFlowJob {
   int tool = 0;
@@ -23,7 +15,7 @@ struct MgpuFlowJob {
   void* out0 = nullptr;
   float* out1 = nullptr;
 };
-// the five sibling sweep tools on row strips; in[] = the further inputs (NULL = not used) and out[] = the outputs (mappings from
+// the sweep tools on row strips; in[] = the further inputs (NULL = not used) and out[] = the outputs (mappings from
 // mgpu_alloc_shared, nx * ny cells of the output's type) of each tool:
 //   EXTREMEUP  d8flowpathextremeup  in: sa                 out: ssa
 //   GRIDNET    gridnet              in: mask (int32)       out: plen, tlen, gord (int16)
@@ -33,8 +25,10 @@ struct MgpuFlowJob {
 //   SLOPEAVEDOWN  slopeavedown      in: fel                out: slpd (the D8 sweep of p, then niter passes at dn)
 //   FLOWDIRCOND   flowdircond       in: z                  out: zfdc
 //   RETLIMFLOW    retlimflow        in: wg, rc             out: qrl
+//   AREAD8        aread8            in: w (or NULL)        out: ad8
+//   AREADINF      areadinf          in: w (or NULL)        out: sca
 struct MgpuSibJob {
-  enum { EXTREMEUP = 0, GRIDNET, DECAY, CONCLIM, TRANSLIM, SLOPEAVEDOWN, FLOWDIRCOND, RETLIMFLOW };
+  enum { EXTREMEUP = 0, GRIDNET, DECAY, CONCLIM, TRANSLIM, SLOPEAVEDOWN, FLOWDIRCOND, RETLIMFLOW, AREAD8, AREADINF, NTOOLS };
   int tool = EXTREMEUP;
   const char* dirfile = nullptr;              // p (D8 tools) or ang
   const char* in[3] = {nullptr, nullptr, nullptr};
@@ -47,9 +41,8 @@ struct MgpuSibJob {
 int mgpu_world();                                // TAUDEM_B200_GPUS (1 = the single-GPU path)
 void* mgpu_alloc_shared(size_t bytes);             // anonymous shared mapping (visible to the forked ranks)
 void mgpu_free_shared(void* p, size_t bytes);
-// runs the job on `world` ranks; compute_seconds = the slowest rank's time from the dependency stencil to the end of the sweep
-int mgpu_area(const MgpuJob& job, int world, double* compute_seconds, int* rounds);
-// the same for a sibling sweep tool (rounds: summed over gridnet's three sweeps; 1 per sweep in peer mode)
+// runs the job on `world` ranks; compute_seconds = the slowest rank's time from the dependency stencil to the end of the sweep;
+// rounds: summed over gridnet's three sweeps, 1 per sweep in peer mode
 int mgpu_sibling(const MgpuSibJob& job, int world, double* compute_seconds, int* rounds);
 // rounds = relaxation / exchange rounds of pitremove, 0 for the flow directions; flats_left = unresolved flat cells of the whole grid
 int mgpu_flow(const MgpuFlowJob& job, int world, double* compute_seconds, int* rounds, long long* flats_left);

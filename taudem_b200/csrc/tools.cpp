@@ -91,30 +91,7 @@ int write_like(const char* name, const Input& like, tdio::DType t, double nodata
 }
 
 // TAUDEM_B200_GPUS=N (N > 1): the reference's `mpiexec -n N <tool>` — one forked process per GPU, each with its row strip
-// (mgpu.cu).  The ranks read their own rows; the parent writes the result.
-int area_multi_gpu(int dinf, int world, const Input& in, const char* infile, const char* wfile, int usew, int contcheck, const char* outfile,
-                   double t0, const char* nproc_label) {
-  const size_t bytes = (size_t)in.nx * in.ny * sizeof(float);
-  float* out = (float*)td::mgpu_alloc_shared(bytes);
-  if (!out) { td::set_error("cannot map the shared output raster"); return TD_ERR_IO; }
-  td::MgpuJob J;
-  J.dinf = dinf; J.dirfile = infile; J.wfile = wfile; J.usew = usew; J.contcheck = contcheck; J.nx = in.nx; J.ny = in.ny; J.out = out;
-  const double t1 = now();
-  double secs = 0.; int rounds = 0;
-  int rc = td::mgpu_area(J, world, &secs, &rounds);
-  const double t2 = now();
-  if (rc) printf("%s device error: %s\n", dinf ? "AreaDinf" : "AreaD8", td_last_error());
-  else rc = write_like(outfile, in, tdio::DT_F32, (double)-1.0f, (const float*)out);
-  const double t3 = now();
-  td::mgpu_free_shared(out, bytes);
-  if (rc) return rc;
-  // (the ranks read their rows inside what the reference calls compute time: Read time is the header pass)
-  printf("%s: %d\nRead time: %f\nCompute time: %f\nWrite time: %f\nTotal time: %f\n", nproc_label, world, t1 - t0, t2 - t1, t3 - t2, t3 - t0);
-  printf("Device compute time: %f\nExchange rounds: %d\n", secs, rounds);
-  return TD_OK;
-}
-
-// the same for pitremove / d8flowdir / dinfflowdir / peukerdouglas (mgpu_flow): the ranks read their rows of the DEM, the parent
+// (mgpu.cu).  pitremove / d8flowdir / dinfflowdir / peukerdouglas (mgpu_flow): the ranks read their rows of the DEM, the parent
 // writes the rasters
 int flow_multi_gpu(int tool, int world, const Input& dem, const char* demfile, const char* maskfile, int use_mask, int four, const char* out0file,
                    const char* out1file, double t0, double t1, const float* par = nullptr) {
@@ -184,11 +161,12 @@ int companion(Input& a, Input& g, const char* file, std::vector<T>* data, tdio::
   return g.read(data, dt);
 }
 
-// TAUDEM_B200_GPUS=N for the five sibling sweep tools (mgpu_sibling): the ranks read their rows of every input, the parent writes
-// the outputs (mapping slot, file, type, nodata) in the order the single-GPU run writes them
+// TAUDEM_B200_GPUS=N for the sweep tools (mgpu_sibling): the ranks read their rows of every input, the parent writes the outputs (mapping
+// slot, file, type, nodata) in the order the single-GPU run writes them; nproc_label heads the process count's line
 bool use_multi_gpu(const Input& in, int useOutlets) { return td::mgpu_world() > 1 && useOutlets != 1 && in.ny >= td::mgpu_world(); }
 struct SibOut { int slot; const char* file; tdio::DType t; double nodata; };
-int sibling_multi_gpu(td::MgpuSibJob& J, const Input& like, const std::vector<SibOut>& outs, double t0, const char* name) {
+int sibling_multi_gpu(td::MgpuSibJob& J, const Input& like, const std::vector<SibOut>& outs, double t0, const char* name,
+                      const char* nproc_label = "Processors") {
   const int world = td::mgpu_world();
   const size_t n = (size_t)like.nx * like.ny;
   size_t bytes[3] = {0, 0, 0};
@@ -211,7 +189,7 @@ int sibling_multi_gpu(td::MgpuSibJob& J, const Input& like, const std::vector<Si
   unmap();
   if (rc) return rc;
   // (the ranks read their rows inside what is reported as compute time: Read time is the header pass)
-  printf("Processors: %d\nRead time: %f\nCompute time: %f\nWrite time: %f\nTotal time: %f\n", world, t1 - t0, t2 - t1, t3 - t2, t3 - t0);
+  printf("%s: %d\nRead time: %f\nCompute time: %f\nWrite time: %f\nTotal time: %f\n", nproc_label, world, t1 - t0, t2 - t1, t3 - t2, t3 - t0);
   printf("Device compute time: %f\nExchange rounds: %d\n", secs, rounds);
   return TD_OK;
 }
@@ -448,14 +426,12 @@ int td_aread8(const char* pfile, const char* afile, const char* datasrc, const c
   if (useOutlets == 1) { if (int rc = outlet_cells(datasrc, lyrname, uselyrname, lyrno, p, &ocols, &orows)) return rc; }
   std::vector<int16_t> dir;
   nodata_msgs(p.r.nodata(), "int16_t", (int16_t)p.r.nodata());
-  if (td::mgpu_world() > 1 && useOutlets != 1 && p.ny >= td::mgpu_world()) {
+  if (use_multi_gpu(p, useOutlets)) {
     Input w;
-    if (usew) {
-      if (int rc = w.open(wfile)) return rc;
-      if (!tdio::compare_rasters(p.r, p.path, w.r, w.path)) { printf("File sizes do not match\n%s\n", wfile); td::set_error("weight grid does not match"); return TD_ERR_MISMATCH; }
-      nodata_msgs(w.r.nodata(), "float", (float)w.r.nodata());
-    }
-    return area_multi_gpu(0, td::mgpu_world(), p, pfile, wfile, usew, contcheck, afile, t0, "Number of Processes");
+    if (usew) { if (int rc = companion_open(p, w, wfile, tdio::DT_F32, "float", "weight grid does not match")) return rc; }
+    td::MgpuSibJob J;
+    J.tool = td::MgpuSibJob::AREAD8; J.dirfile = pfile; J.in[0] = usew ? wfile : nullptr; J.contcheck = contcheck;
+    return sibling_multi_gpu(J, p, {{0, afile, tdio::DT_F32, (double)-1.0f}}, t0, "AreaD8", "Number of Processes");
   }
   Warmup warm;
   if (int rc = p.read(&dir, tdio::DT_I16)) return rc;
@@ -497,14 +473,16 @@ int td_area(const char* angfile, const char* scafile, const char* datasrc, const
   if (useOutlets == 1) { if (int rc = outlet_cells(datasrc, lyrname, uselyrname, lyrno, a, &ocols, &orows)) return rc; }
   std::vector<float> ang;
   nodata_msgs(a.r.nodata(), "float", (float)a.r.nodata());
-  if (td::mgpu_world() > 1 && useOutlets != 1 && a.ny >= td::mgpu_world()) {
+  if (use_multi_gpu(a, useOutlets)) {
     Input w;
     if (usew) {
       if (int rc = w.open(wfile)) return rc;
       if (!tdio::compare_rasters(a.r, a.path, w.r, w.path)) { td::set_error("weight grid does not match"); return TD_ERR_ARG; }
       nodata_msgs(w.r.nodata(), "float", (float)w.r.nodata());
     }
-    return area_multi_gpu(1, td::mgpu_world(), a, angfile, wfile, usew, contcheck, scafile, t0, "Processors");
+    td::MgpuSibJob J;
+    J.tool = td::MgpuSibJob::AREADINF; J.dirfile = angfile; J.in[0] = usew ? wfile : nullptr; J.contcheck = contcheck;
+    return sibling_multi_gpu(J, a, {{0, scafile, tdio::DT_F32, (double)-1.0f}}, t0, "AreaDinf");
   }
   Warmup warm;
   if (int rc = a.read(&ang, tdio::DT_F32)) return rc;

@@ -178,6 +178,23 @@ int td_lengtharea_host(const float* plen, const int32_t* ad8, int16_t* ss, int n
 int td_sloped(const char* pfile, const char* felfile, const char* slpdfile, double dn);
 int td_slopeavedown_host(const float* fel, const int16_t* p, float* slpd, int nx, int ny, float fel_nodata, int16_t p_nodata, const double* dxc,
                          const double* dyc, double dx, double dy, double dn);
+/* d8hdisttostrm / d8vdisttostrm: the distance from every cell down its D8 path to the first stream cell (src >= thresh where src,
+ * read as int32, is data), horizontal (the path length) or vertical (the drop: height above the nearest drainage).  File level =
+ * `int distgrid(char* pfile, char* srcfile, char* distfile, int thresh)` (src/D8HDistToStrm.cpp:57) and `int d8vdistdown(char*
+ * pfile, char* felfile, char* srcfile, char* distfile, int thresh)` (src/D8VDistToStrm.cpp:58); TD_ERR_MISMATCH, after "File sizes
+ * do not match", when src or fel differs from p in size.  dist: float32, nodata MISSINGFLOAT, the georeference of p.  Stream cells
+ * get 0; cells whose path leaves the grid, meets a non-stream cell whose p is nodata, 0 or outside 1..8, or ends in a cycle without
+ * a stream cell keep MISSINGFLOAT.  Host-grid level: dxc / dyc = per-row cell sizes (horizontal only).  One GPU takes a grid whose
+ * strip, (ny + 2) * td_pitch_for(nx) cells, holds fewer than 2^32 cells (TD_ERR_ARG otherwise) and whose rasters fit its memory: 15
+ * bytes per strip cell (horizontal; 19 vertical).  Bit-exact.  td_disttostrm_last_levels: the
+ * BFS levels of the last host-grid call. */
+int td_distgrid(const char* pfile, const char* srcfile, const char* distfile, int thresh);
+int td_d8vdistdown(const char* pfile, const char* felfile, const char* srcfile, const char* distfile, int thresh);
+int td_d8hdisttostrm_host(const int16_t* p, const int32_t* src, float* dist, int nx, int ny, int16_t p_nodata, int32_t src_nodata, int thresh,
+                          const double* dxc, const double* dyc);
+int td_d8vdisttostrm_host(const int16_t* p, const float* fel, const int32_t* src, float* dist, int nx, int ny, int16_t p_nodata, int32_t src_nodata,
+                          int thresh);
+long long td_disttostrm_last_levels(void);
 /* flowdircond: D8-conditioned elevations.  Every cell the D8 queue of p reaches gets the smallest conditioned elevation among the
  * cells that drain into it, or its own z if that is smaller, so that elevations never rise downstream along p; the other cells keep
  * their z.  A cell whose z is nodata keeps it and still drains.  File level = `int flowdircond(char* pfile, char* zfile, char*
@@ -416,6 +433,18 @@ int td_slopeavedown_init_dev(td_ctx*, const int16_t* p, const float* fel, uint8_
 int td_slopeavedown_pass_dev(td_ctx*, const uint8_t* code, const float* fel, const float* ed_dd_in, float* ed_dd_out, float* sd, td_strip s,
                              const float* dist, double dn, int* changed, void* stream);
 int td_slopeavedown_niter(double dn, double dx, double dy, int* niter);
+/* d8hdisttostrm / d8vdisttostrm on a strip (disttostrm.cu).  td_disttostrm_seed_dev writes dist (MISSINGFLOAT, 0 on the owned stream
+ * cells) and code (one byte per strip cell) and starts the BFS frontier with the stream cells; td_disttostrm_levels_dev first gives
+ * the owned edge-row cells whose receiver lies in a halo row of dist that holds a value their values, then runs BFS levels until the
+ * frontier is empty (a batch of levels per host read-back).  vertical = 0: rowdist = the device table of the strip's own rows
+ * (td_slopeavedown_pass_dev's dist); vertical = 1: fel with valid halo rows.  On row strips the caller copies the first / last owned
+ * rows of dist into the neighbours' halo rows after each levels call and repeats until no strip added a cell: *cells (may be NULL) =
+ * the cells that joined the frontier since the previous call, the seeds included; *levels (may be NULL) = the non-empty levels run.
+ * The frontier lives on the context (its listA / listB): nothing else may run on it between the seed and the last levels call. */
+int td_disttostrm_seed_dev(td_ctx*, const int16_t* p, const int32_t* src, float* dist, uint8_t* code, td_strip s, int thresh, int16_t p_nodata,
+                           int32_t src_nodata, void* stream);
+int td_disttostrm_levels_dev(td_ctx*, int vertical, const uint8_t* code, const float* fel, const float* rowdist, float* dist, td_strip s,
+                             unsigned long long* cells, long long* levels, void* stream);
 
 /* Peer mode (one process per GPU on one NVSwitch box): every rank exports the IPC handles of the buffers
  * its neighbours write (counts, tile scheduler, halo areas, rank 0 also the global pending counter), opens

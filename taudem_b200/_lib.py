@@ -73,6 +73,13 @@ SIGNATURES = {
     "td_slopeavedown_init_dev": (_I, [_P, _P, _P, _P, _P, _P, _P, Strip, C.c_int16, _F, _P]),
     "td_slopeavedown_pass_dev": (_I, [_P, _P, _P, _P, _P, _P, Strip, _P, _D, _P, _P]),
     "td_slopeavedown_niter": (_I, [_D, _D, _D, _P]),
+    "td_distgrid": (_I, [_S, _S, _S, _I]),
+    "td_d8vdistdown": (_I, [_S, _S, _S, _S, _I]),
+    "td_d8hdisttostrm_host": (_I, [_P, _P, _P, _I, _I, C.c_int16, C.c_int32, _I, _P, _P]),
+    "td_d8vdisttostrm_host": (_I, [_P, _P, _P, _P, _I, _I, C.c_int16, C.c_int32, _I]),
+    "td_disttostrm_last_levels": (C.c_longlong, []),
+    "td_disttostrm_seed_dev": (_I, [_P, _P, _P, _P, _P, Strip, _I, C.c_int16, C.c_int32, _P]),
+    "td_disttostrm_levels_dev": (_I, [_P, _I, _P, _P, _P, _P, Strip, _P, _P, _P]),
     "td_flowdircond": (_I, [_S, _S, _S]),
     "td_flowdircond_host": (_I, [_P, _P, _P, _I, _I, C.c_int16, _F]),
     "td_flowdircond_deps_dev": (_I, [_P, _P, _P, _P, Strip, C.c_int16, _P]),

@@ -322,6 +322,42 @@ def slopeavedown_grid(fel, p, dn=50.0, dx=30.0, dy=30.0, nodata=float(FEL_NODATA
     return slpd
 
 
+def _stream_args(p, src, what):
+    p = _grid(p, np.int16)
+    src = _grid(src, np.int32)
+    if src.shape != p.shape:
+        raise ValueError(f"{what}: p and src differ in shape")
+    return p, src
+
+
+def d8hdisttostrm_grid(p, src, thresh=1, dx=30.0, dy=30.0, p_nodata=int(MISSINGSHORT), src_nodata=-2147483648, dxc=None, dyc=None):
+    """D8 horizontal distance down to the stream (td_d8hdisttostrm_host; src/D8HDistToStrm.cpp:57-226): the length of every cell's D8
+    path to the first stream cell (src >= thresh where src, read as int32, is not src_nodata), float32, 0 on the stream, nodata
+    MISSINGFLOAT where the path never reaches one.  dxc / dyc: per-row cell sizes (default dx / dy on every row)."""
+    p, src = _stream_args(p, src, "d8hdisttostrm_grid")
+    ny, nx = p.shape
+    dxc = _rows(dx if dxc is None else dxc, ny)
+    dyc = _rows(dy if dyc is None else dyc, ny)
+    dist = np.empty((ny, nx), np.float32)
+    check(lib().td_d8hdisttostrm_host(_ptr(p), _ptr(src), _ptr(dist), nx, ny, int(p_nodata), int(src_nodata), int(thresh), _ptr(dxc), _ptr(dyc)))
+    return dist
+
+
+def d8vdisttostrm_grid(p, fel, src, thresh=1, p_nodata=int(MISSINGSHORT), src_nodata=-2147483648):
+    """D8 vertical distance down to the stream, the height above the nearest drainage (td_d8vdisttostrm_host;
+    src/D8VDistToStrm.cpp:58-240): fel minus the elevation of the first stream cell down every cell's D8 path, summed step by step in
+    float32 as the reference does, 0 on the stream, nodata MISSINGFLOAT where the path never reaches one.  fel's nodata is not
+    tested: its values go through the arithmetic."""
+    p, src = _stream_args(p, src, "d8vdisttostrm_grid")
+    fel = _grid(fel, np.float32)
+    if fel.shape != p.shape:
+        raise ValueError("d8vdisttostrm_grid: p and fel differ in shape")
+    ny, nx = p.shape
+    dist = np.empty((ny, nx), np.float32)
+    check(lib().td_d8vdisttostrm_host(_ptr(p), _ptr(fel), _ptr(src), _ptr(dist), nx, ny, int(p_nodata), int(src_nodata), int(thresh)))
+    return dist
+
+
 def flowdircond_grid(p, z, p_nodata=int(MISSINGSHORT), nodata=-9999.0):
     """D8-conditioned elevations (td_flowdircond_host; src/flowdircond.cpp:143-194): every cell the aread8 queue of `p` reaches gets
     the smallest conditioned elevation among the cells that drain into it, or its own z if that is smaller, so that elevations never

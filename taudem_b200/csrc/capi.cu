@@ -1006,6 +1006,82 @@ int td_slopeavedown_host(const float* fel, const int16_t* p, float* slpd, int nx
   });
 }
 
+// ---- d8hdisttostrm / d8vdisttostrm (disttostrm.cu): the BFS from the stream cells, one level per launch
+namespace {
+long long g_dts_levels = 0;
+// the frontier list (listA, one 4-byte entry per strip cell), the level bounds and the block counter (listB), the append / consume
+// counters (d_ctr[37], [38])
+int dts_bufs(td_ctx* ctx, const Strip& s, td::DtsBufs* b) {
+  TD_CUDA(ctx->listA.ensure(sizeof(unsigned) * (size_t)s.cells()));
+  TD_CUDA(ctx->listB.ensure(sizeof(unsigned long long) * (td::DTS_BATCH + 3)));
+  b->list = ctx->listA.as<unsigned>();
+  b->ctr = ctx->d_ctr + 37;
+  b->bounds = ctx->listB.as<unsigned long long>();
+  b->blkdone = reinterpret_cast<unsigned*>(b->bounds + td::DTS_BATCH + 2);
+  return TD_OK;
+}
+}  // namespace
+int td_disttostrm_seed_dev(td_ctx* ctx, const int16_t* p, const int32_t* src, float* dist, uint8_t* code, td_strip s, int thresh, int16_t p_nodata,
+                           int32_t src_nodata, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  if (!ctx || !p || !src || !dist || !code || Strip(s).cells() >= (1ll << 32)) {
+    td::set_error("td_disttostrm_seed_dev: bad arguments (a strip holds fewer than 2^32 cells, halo rows and padding included)");
+    return TD_ERR_ARG;
+  }
+  td::DtsBufs b;
+  if (int rc = dts_bufs(ctx, Strip(s), &b)) return rc;
+  return td::dts_seed(p, src, dist, code, Strip(s), thresh, p_nodata, src_nodata, b, (cudaStream_t)stream);
+}
+int td_disttostrm_levels_dev(td_ctx* ctx, int vertical, const uint8_t* code, const float* fel, const float* rowdist, float* dist, td_strip s,
+                             unsigned long long* cells, long long* levels, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  if (!ctx || !code || !dist || (vertical ? !fel : !rowdist) || Strip(s).cells() >= (1ll << 32) || ctx->listA.cap < sizeof(unsigned) * (size_t)Strip(s).cells()) {
+    td::set_error("td_disttostrm_levels_dev: bad arguments (td_disttostrm_seed_dev of this strip comes first, on this context)");
+    return TD_ERR_ARG;
+  }
+  td::DtsBufs b;
+  if (int rc = dts_bufs(ctx, Strip(s), &b)) return rc;
+  int dev = 0, sms = 1;
+  TD_CUDA(cudaGetDevice(&dev));
+  TD_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  return td::dts_levels(vertical != 0, code, fel, rowdist, dist, Strip(s), b, sms * 4, cells, levels, (cudaStream_t)stream);
+}
+long long td_disttostrm_last_levels(void) { return g_dts_levels; }
+}  // extern "C"
+
+namespace {
+// src/D8HDistToStrm.cpp:57-226 / src/D8VDistToStrm.cpp:58-240 on one strip
+int dts_host(const char* who, bool vertical, const int16_t* p, const float* fel, const int32_t* src, float* dist, int nx, int ny, int16_t p_nodata,
+             int32_t src_nodata, int thresh, const double* dxc, const double* dyc) {
+  const bool ok = p && src && dist && (vertical ? fel != nullptr : (dxc && dyc));
+  return host_call(who, ok && (long long)(ny + 2) * td_pitch_for(nx) < (1ll << 32), nx, ny, [&](HostGrid& g) {
+    const float* d_rd = vertical ? nullptr : g.dist(dxc, dyc);
+    const int16_t* d_p = g.in(p);
+    const int32_t* d_src = g.in(src);
+    const float* d_fel = vertical ? g.in(fel) : nullptr;
+    float* d_dist = g.alloc<float>();
+    uint8_t* d_code = g.alloc<uint8_t>();
+    g.start();
+    HG_TD(td_disttostrm_seed_dev(g.ctx, d_p, d_src, d_dist, d_code, g.s, thresh, p_nodata, src_nodata, g.st));
+    long long levels = 0;
+    HG_TD(td_disttostrm_levels_dev(g.ctx, vertical, d_code, d_fel, d_rd, d_dist, g.s, nullptr, &levels, g.st));
+    g_dts_levels = levels;
+    g.stop();
+    g.down(dist, d_dist);
+  }, " (fewer than 2^32 strip cells)");
+}
+}  // namespace
+
+extern "C" {
+int td_d8hdisttostrm_host(const int16_t* p, const int32_t* src, float* dist, int nx, int ny, int16_t p_nodata, int32_t src_nodata, int thresh,
+                          const double* dxc, const double* dyc) {
+  return dts_host("td_d8hdisttostrm_host", false, p, nullptr, src, dist, nx, ny, p_nodata, src_nodata, thresh, dxc, dyc);
+}
+int td_d8vdisttostrm_host(const int16_t* p, const float* fel, const int32_t* src, float* dist, int nx, int ny, int16_t p_nodata, int32_t src_nodata,
+                          int thresh) {
+  return dts_host("td_d8vdisttostrm_host", true, p, fel, src, dist, nx, ny, p_nodata, src_nodata, thresh, nullptr, nullptr);
+}
+
 // aread8 + areadinf of one DEM in ONE call with the copies overlapped with the kernels: three streams — host -> device (p, then
 // ang), compute (aread8 as soon as p has arrived, areadinf as soon as ang has and aread8 is done), device -> host (ad8 while
 // areadinf runs, then sca).  Same kernels, same results as td_aread8_host followed by td_area_host (no weights, no outlets).

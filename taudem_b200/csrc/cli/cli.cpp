@@ -1,5 +1,6 @@
 // Command line front ends: pitremove, d8flowdir, dinfflowdir, aread8, areadinf (+ the point-wise consumers threshold, twi, slopearea, slopearearatio,
-// the sibling sweep tools, the stream definitions peukerdouglas and lengtharea, slopeavedown, flowdircond and retlimflow).
+// the sibling sweep tools, the stream definitions peukerdouglas and lengtharea, slopeavedown, flowdircond, retlimflow, d8hdisttostrm and
+// d8vdisttostrm).
 // Same flags, same two invocation styles and the same "print usage and exit(0)" error
 // behaviour as the reference mains (src/PitRemovemn.cpp:48-172, src/D8FlowDirmn.cpp:49-146,
 // src/DinfFlowDirmn.cpp:54-147, src/aread8mn.cpp:49-193, src/areadinfmn.cpp:49-178);
@@ -565,6 +566,50 @@ int main(int argc, char** argv) {
   if (argc == 2) { td_nameadd(ang, argv[1], "ang"); td_nameadd(rc, argv[1], "rc"); td_nameadd(qrl, argv[1], "qrl"); td_nameadd(wg, argv[1], "wg"); }
   int err = td_retlimro(ang, wg, rc, qrl) != 0;
   if (err) printf("RetlimFlow error %d\n", err);
+  return done();
+}
+#elif defined(TOOL_d8hdisttostrm) || defined(TOOL_d8vdisttostrm)
+// src/D8HDistToStrmmn.cpp:51-149 and src/D8VDistToStrmmn.cpp:52-163 (the reference's usage texts; -thresh is read with %d, default 1).
+// Their error line always shows 1 (`err=distgrid(...) != 0` assigns the comparison).  Rasters whose sizes differ end the program
+// with exit status 5 after "File sizes do not match", as the reference's MPI_Abort(MCW, 5) does.
+#if defined(TOOL_d8vdisttostrm)
+#define DTS_V 1
+#else
+#define DTS_V 0
+#endif
+static void usage(const char* prog) {
+  printf("Simple Usage:\n %s <basefilename>\n", prog);
+  printf("Usage with specific file names:\n %s -p <pfile>\n", prog);
+  printf(DTS_V ? "-fel <felfile> -src <srcfile> -dist <distfile> [-thresh <thresh>]\n" : "-src <srcfile> -dist <distfile> [-thresh <thresh>]\n");
+  printf("<basefilename> is the name of the base digital elevation model\n");
+  printf("<pfile> is the d8 flow direction input file.\n");
+  if (DTS_V) printf("<felfile> is the pit filled or carved elevation input file.\n");
+  printf("<srcfile> is the stream raster input file.\n");
+  printf(DTS_V ? "<distfile> is the vertical distance to stream output file.\n" : "<distfile> is the distance to stream output file.\n");
+  printf("The optional <thresh> is the user input threshold number.\n");
+  printf("The following are appended to the file names\n");
+  printf("before the files are opened:\n");
+  printf("p      D8 flow directions (input)\n");
+  if (DTS_V) printf("fel    pit filled or carved elevation file\n");
+  printf("src    stream raster file (Input)\n");
+  printf("dist   distance to stream file(output)\n");
+  exit(0);
+}
+int main(int argc, char** argv) {
+  static char p[MAXLN], fel[MAXLN], src[MAXLN], dist[MAXLN];
+  int thresh = 1;
+  Opt opts[] = {{"-p", 0, p, NULL, 0}, {"-src", 0, src, NULL, 0}, {"-dist", 0, dist, NULL, 0}, {"-thresh", 2, NULL, &thresh, 0}, {"-fel", 0, fel, NULL, 0}};
+  parse(argc, argv, opts, DTS_V ? 5 : 4);
+  if (argc == 2) {
+    td_nameadd(p, argv[1], "p");
+    if (DTS_V) td_nameadd(fel, argv[1], "fel");
+    td_nameadd(src, argv[1], "src");
+    td_nameadd(dist, argv[1], "dist");
+  }
+  const int rc = DTS_V ? td_d8vdistdown(p, fel, src, dist, thresh) : td_distgrid(p, src, dist, thresh);
+  if (rc == TD_ERR_MISMATCH) { fflush(stdout); _exit(5); }
+  const int err = rc != 0;
+  if (err) printf(DTS_V ? "D8 distance down error %d\n" : "D8 distance error %d\n", err);
   return done();
 }
 #else

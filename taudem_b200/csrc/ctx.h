@@ -52,7 +52,8 @@ struct td_ctx {
   static constexpr int SWEEP_KERNELS = 16;   // instantiations of the warp-per-tile sweep kernel (the table SWEEPS in sweep_warp.cu)
   int wgrid[SWEEP_KERNELS] = {0};         // persistent grid of each of them on this context's device
   static constexpr int NCTR = 40;        // device counters: [24..32] the contributing-area sweep's statistics (sweep_warp.cu WArgs::stat),
-                                         // [36] slopeavedown's changed flag (capi.cu)
+                                         // [36] slopeavedown's changed flag, [37..38] the disttostrm frontier's
+                                         // appended / consumed entries (capi.cu)
   unsigned long long* d_ctr = nullptr;   // NCTR device counters
   unsigned long long* h_ctr = nullptr;   // pinned host mirror
   td_ctx();

@@ -61,6 +61,16 @@ int launch_sad_init(const short* p, const unsigned char* cnt, const float* fel, 
                     const Strip& s, short p_nodata, float fel_nodata, cudaStream_t st);
 int launch_sad_pass(const unsigned char* code, const float* fel, const float* src, float* dst, float* sd, const float* dist, const Strip& s,
                     double dn, int* changed, cudaStream_t st);
+// disttostrm.cu: the BFS from the stream cells of d8hdisttostrm / d8vdisttostrm.  list: one entry per strip cell at most;
+// ctr[0] = entries appended, ctr[1] = entries consumed by the levels run so far; bounds: DTS_BATCH + 2 words; blkdone: one word.
+constexpr int DTS_BATCH = 64;     // BFS levels per host read-back
+struct DtsBufs { unsigned* list; unsigned long long* ctr; unsigned long long* bounds; unsigned* blkdone; };
+int dts_seed(const short* p, const int* src, float* val, unsigned char* code, const Strip& s, int thresh, short p_nodata, int src_nodata,
+             const DtsBufs& b, cudaStream_t st);
+// the edge-row cells of a row strip whose receiver is in a halo row with a value, then levels until the frontier is empty (grid
+// blocks per level); *cells = the list entries added since the last call (with the seeds), *levels = the non-empty levels run
+int dts_levels(bool vertical, const unsigned char* code, const float* fel, const float* dist, float* val, const Strip& s, const DtsBufs& b, int grid,
+               unsigned long long* cells, long long* levels, cudaStream_t st);
 int launch_mask_ok(const int* mask, float* ok, const Strip& s, int thresh, cudaStream_t st);
 int launch_gord_finish(const float* g, const short* p, const float* ok, const unsigned short* node, short* gord, const Strip& s, short p_nodata,
                        int outlets, cudaStream_t st);

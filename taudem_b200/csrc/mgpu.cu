@@ -1,6 +1,7 @@
 // Multi-GPU sweeps behind the executables: `TAUDEM_B200_GPUS=N aread8 ...` / `areadinf ...`, and the same for d8flowpathextremeup,
-// gridnet, dinfdecayaccum, dinfconclimaccum, dinftranslimaccum, slopeavedown (whose passes follow its D8 sweep there), flowdircond
-// and retlimflow: sibling_worker.  pitremove, d8flowdir, dinfflowdir and peukerdouglas: flow_worker.
+// gridnet, dinfdecayaccum, dinfconclimaccum, dinftranslimaccum, slopeavedown (whose passes follow its D8 sweep there), flowdircond,
+// retlimflow, d8hdisttostrm and d8vdisttostrm (a BFS from the stream cells there): sibling_worker.  pitremove, d8flowdir,
+// dinfflowdir and peukerdouglas: flow_worker.
 //
 // reference: the callers' contract is `mpiexec -n N aread8` (src/aread8.cpp:57,100: MPI_Init, one row strip per rank,
 // src/linearpart.h:160-200 the partition, src/aread8.cpp:280-304 the border exchange + ringTerm loop).  Here the
@@ -207,6 +208,8 @@ const SibTool sib_tools[MgpuSibJob::NTOOLS] = {
     {true, {F32, F32, F32}},             // RETLIMFLOW
     {false, {F32, F32, F32}},            // AREAD8
     {true, {F32, F32, F32}},             // AREADINF
+    {false, {tdio::DT_I32, F32, F32}},   // D8HDIST
+    {false, {tdio::DT_I32, F32, F32}},   // D8VDIST
 };
 
 void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int world) {
@@ -246,7 +249,7 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
   }
   // the travelling value, the other outputs, gridnet's mask grid / distances / orders, the halo counts
   float *d_val = nullptr, *d_dep = nullptr, *d_co = nullptr, *d_ok = nullptr, *d_dist = nullptr; int16_t* d_g = nullptr; int* d_halo = nullptr;
-  uint8_t* d_code = nullptr; float* d_state[2] = {nullptr, nullptr};                      // slopeavedown
+  uint8_t* d_code = nullptr; float* d_state[2] = {nullptr, nullptr};                      // slopeavedown (d_code: and disttostrm)
   double* d_dx = nullptr;
   MG_CUDA(cudaMalloc(&d_val, cells * 4));
   MG_CUDA(cudaMalloc(&d_halo, sizeof(int) * 4 * (size_t)s.pitch));        // halo_out (2 pitch) + the received decrements (2 pitch)
@@ -256,7 +259,7 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
   }
   std::vector<double> dxc, dyc;
   in.cell_sizes(&dxc, &dyc);
-  if (J.tool == MgpuSibJob::GRIDNET || J.tool == MgpuSibJob::SLOPEAVEDOWN) {
+  if (J.tool == MgpuSibJob::GRIDNET || J.tool == MgpuSibJob::SLOPEAVEDOWN || J.tool == MgpuSibJob::D8HDIST) {
     if (J.tool == MgpuSibJob::GRIDNET) {
       if (J.in[0]) MG_CUDA(cudaMalloc(&d_ok, cells * 4));
       MG_CUDA(cudaMalloc(&d_g, cells * 2));
@@ -369,6 +372,32 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
         ++rounds;
         MG_BAR();
         if (any == 0) break;                                  // no rank changed anything: the remaining passes would not either
+      }
+      break;
+    }
+    case MgpuSibJob::D8HDIST:
+    case MgpuSibJob::D8VDIST: {
+      // the reference's ring loop (src/D8HDistToStrm.cpp:158-226): BFS levels until the strip's frontier is empty, the value raster's
+      // edge rows to the neighbours (fdarr->share()), and the owned edge-row cells whose receiver just got a value start the next
+      // levels; until no rank added a cell (ringTerm)
+      MG_CUDA(cudaMalloc(&d_code, cells));
+      MG_TD(td_disttostrm_seed_dev(ctx, (const int16_t*)d_dir, (const int32_t*)d_in[0], d_val, d_code, s, J.thresh, p_nd, (int32_t)rin[0].nodata(), st));
+      const RoundBuf R{extra, s.pitch};
+      const size_t rb = sizeof(float) * (size_t)s.pitch;
+      for (;;) {
+        unsigned long long added = 0;
+        MG_TD(td_disttostrm_levels_dev(ctx, J.tool == MgpuSibJob::D8VDIST, d_code, f1, d_dist, d_val, s, &added, nullptr, st));
+        MG_CUDA(cudaMemcpy(R.row(rank, 0), d_val + s.pitch, rb, cudaMemcpyDeviceToHost));
+        MG_CUDA(cudaMemcpy(R.row(rank, 1), d_val + (size_t)ny * s.pitch, rb, cudaMemcpyDeviceToHost));
+        S->red[rank][0] = added;
+        MG_BAR();
+        unsigned long long any = 0;
+        for (int r = 0; r < world; ++r) any += S->red[r][0];
+        if (rank > 0) MG_CUDA(cudaMemcpy(d_val, R.row(rank - 1, 1), rb, cudaMemcpyHostToDevice));
+        if (rank < world - 1) MG_CUDA(cudaMemcpy(d_val + (size_t)(ny + 1) * s.pitch, R.row(rank + 1, 0), rb, cudaMemcpyHostToDevice));
+        ++rounds;
+        MG_BAR();
+        if (any == 0) break;                                  // nobody added a cell: every edge row is final
       }
       break;
     }

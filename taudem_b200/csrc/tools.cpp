@@ -1043,4 +1043,58 @@ int td_retlimro(const char* angfile, const char* wgfile, const char* rcfile, con
   return TD_ERR_IO;
 }
 
+// src/D8HDistToStrm.cpp:57-226 / src/D8VDistToStrm.cpp:58-240: p (int16), fel (float, vertical only) and src (int32) in, dist out
+// (float32, nodata MISSINGFLOAT, the georeference of p).  The horizontal distances use p's per-row cell sizes.  TAUDEM_B200_GPUS=N
+// runs it on N row strips.
+static int disttostrm(bool vertical, const char* pfile, const char* felfile, const char* srcfile, const char* distfile, int thresh) try {
+  const char* name = vertical ? "D8VDistToStrm" : "D8HDistToStrm";
+  printf("%s version %s\n", name, td_version());
+  fflush(stdout);
+  const double t0 = now();
+  Input p;
+  if (int rc = p.open(pfile)) return rc;
+  nodata_msgs(p.r.nodata(), "int16_t", (int16_t)p.r.nodata());
+  Input z, g;
+  if (vertical) { if (int rc = companion_open(p, z, felfile, tdio::DT_F32, "float", "elevation grid does not match")) return rc; }
+  if (int rc = companion_open(p, g, srcfile, tdio::DT_I32, "int32_t", "stream raster does not match")) return rc;
+  if (use_multi_gpu(p, 0)) {
+    td::MgpuSibJob J;
+    J.tool = vertical ? td::MgpuSibJob::D8VDIST : td::MgpuSibJob::D8HDIST; J.dirfile = pfile; J.in[0] = srcfile; J.in[1] = vertical ? felfile : nullptr;
+    J.thresh = thresh;
+    return sibling_multi_gpu(J, p, {{0, distfile, tdio::DT_F32, (double)-3.4028234663852886e38f}}, t0, name);
+  }
+  Warmup warm;
+  std::vector<int16_t> dir;
+  std::vector<float> fel;
+  std::vector<int32_t> src;
+  if (int rc = p.read(&dir, tdio::DT_I16)) return rc;
+  if (vertical) { if (int rc = z.read(&fel, tdio::DT_F32)) return rc; }
+  if (int rc = g.read(&src, tdio::DT_I32)) return rc;
+  warm.join();
+  const double t1 = now();
+  std::vector<float> dist((size_t)p.nx * p.ny);
+  const int rc = vertical ? td_d8vdisttostrm_host(dir.data(), fel.data(), src.data(), dist.data(), p.nx, p.ny, (int16_t)p.r.nodata(), (int32_t)g.r.nodata(), thresh)
+                          : td_d8hdisttostrm_host(dir.data(), src.data(), dist.data(), p.nx, p.ny, (int16_t)p.r.nodata(), (int32_t)g.r.nodata(), thresh,
+                                                  p.dxc.data(), p.dyc.data());
+  if (rc) {
+    printf("%s device error: %s\n", name, td_last_error());
+    return rc;
+  }
+  const double t2 = now();
+  if (int rc2 = write_like(distfile, p, tdio::DT_F32, (double)-3.4028234663852886e38f, dist)) return rc2;
+  const double t3 = now();
+  printf("Processors: 1\nRead time: %f\nCompute time: %f\nWrite time: %f\nTotal time: %f\n", t1 - t0, t2 - t1, t3 - t2, t3 - t0);
+  printf("Device compute time: %f\n", td_last_compute_seconds());
+  return TD_OK;
+} catch (const std::exception& e) {
+  td::set_error(std::string("exception: ") + e.what());
+  return TD_ERR_IO;
+}
+int td_distgrid(const char* pfile, const char* srcfile, const char* distfile, int thresh) {
+  return disttostrm(false, pfile, nullptr, srcfile, distfile, thresh);
+}
+int td_d8vdistdown(const char* pfile, const char* felfile, const char* srcfile, const char* distfile, int thresh) {
+  return disttostrm(true, pfile, felfile, srcfile, distfile, thresh);
+}
+
 }  // extern "C"

@@ -518,7 +518,7 @@ void flow_worker(const MgpuFlowJob& J, Shared* S, char* extra, int rank, int wor
       if (C.allreduce_sum(&any, 1)) throw Fail{"all-reduce failed"};
       if (any == 0) break;
     }
-    MG_CUDA(cudaMemcpy2D((float*)J.out0 + (size_t)row0 * nx, (size_t)nx * 4, d_f + s.pitch, (size_t)s.pitch * 4, (size_t)nx * 4, (size_t)ny, cudaMemcpyDeviceToHost));
+    MG_CUDA(cudaMemcpy2D((float*)J.out[0] + (size_t)row0 * nx, (size_t)nx * 4, d_f + s.pitch, (size_t)s.pitch * 4, (size_t)nx * 4, (size_t)ny, cudaMemcpyDeviceToHost));
   } else if (J.tool == 3) {
     // peukerdouglas: smoothing on the raw halo rows, the smoothed edge rows to the neighbours (src/PeukerDouglas.cpp:165), marks
     MG_CUDA(cudaMalloc(&d_f, cells * 4));
@@ -530,7 +530,7 @@ void flow_worker(const MgpuFlowJob& J, Shared* S, char* extra, int rank, int wor
     MG_TD(td_peukerdouglas_mark_dev(ctx, d_f, (int16_t*)d_dir, s, (float)in.nodata(), st));
     MG_CUDA(cudaStreamSynchronize(st));
     rounds = 1;
-    MG_CUDA(cudaMemcpy2D((int16_t*)J.out0 + (size_t)row0 * nx, (size_t)nx * 2, (int16_t*)d_dir + s.pitch, (size_t)s.pitch * 2, (size_t)nx * 2, (size_t)ny,
+    MG_CUDA(cudaMemcpy2D((int16_t*)J.out[0] + (size_t)row0 * nx, (size_t)nx * 2, (int16_t*)d_dir + s.pitch, (size_t)s.pitch * 2, (size_t)nx * 2, (size_t)ny,
                          cudaMemcpyDeviceToHost));
   } else {
     const bool dinf = J.tool == 2;
@@ -558,9 +558,9 @@ void flow_worker(const MgpuFlowJob& J, Shared* S, char* extra, int rank, int wor
       else MG_TD(td_d8_flats_strip_dev(ctx, d_z, (int16_t*)d_dir, s, d_dx, d_dx + ny, &left, &comm, st));
       MG_CUDA(cudaStreamSynchronize(st));
     }
-    MG_CUDA(cudaMemcpy2D((char*)J.out0 + (size_t)row0 * nx * eb, (size_t)nx * eb, (char*)d_dir + (size_t)s.pitch * eb, (size_t)s.pitch * eb, (size_t)nx * eb, (size_t)ny,
+    MG_CUDA(cudaMemcpy2D((char*)J.out[0] + (size_t)row0 * nx * eb, (size_t)nx * eb, (char*)d_dir + (size_t)s.pitch * eb, (size_t)s.pitch * eb, (size_t)nx * eb, (size_t)ny,
                          cudaMemcpyDeviceToHost));
-    MG_CUDA(cudaMemcpy2D(J.out1 + (size_t)row0 * nx, (size_t)nx * 4, d_slp + s.pitch, (size_t)s.pitch * 4, (size_t)nx * 4, (size_t)ny, cudaMemcpyDeviceToHost));
+    MG_CUDA(cudaMemcpy2D((float*)J.out[1] + (size_t)row0 * nx, (size_t)nx * 4, d_slp + s.pitch, (size_t)s.pitch * 4, (size_t)nx * 4, (size_t)ny, cudaMemcpyDeviceToHost));
   }
   S->secs[rank] = now() - t0;
   if (rank == 0) { S->rounds = rounds; S->flats_left = left; }
@@ -661,7 +661,7 @@ int mgpu_sibling(const MgpuSibJob& J, int world, double* compute_seconds, int* r
 int mgpu_flow(const MgpuFlowJob& J, int world, double* compute_seconds, int* rounds, long long* flats_left) {
   if (world < 2 || world > MAXR) { set_error("mgpu_flow: between 2 and 64 ranks"); return TD_ERR_ARG; }
   if (J.ny < world) { set_error("mgpu_flow: fewer rows than ranks"); return TD_ERR_ARG; }
-  if (J.tool < 0 || J.tool > 3 || !J.out0 || ((J.tool == 1 || J.tool == 2) && !J.out1)) { set_error("mgpu_flow: bad job"); return TD_ERR_ARG; }
+  if (J.tool < 0 || J.tool > 3 || !J.out[0] || ((J.tool == 1 || J.tool == 2) && !J.out[1])) { set_error("mgpu_flow: bad job"); return TD_ERR_ARG; }
   const int pitch = td_pitch_for(J.nx);
   return run_ranks("mgpu_flow", world, RowSlots::bytes(pitch) * (size_t)world,
                    [&](Shared* S, char* extra, int r) { flow_worker(J, S, extra, r, world); }, compute_seconds, rounds, flats_left);

@@ -3,8 +3,9 @@
 #include <stddef.h>
 
 namespace td {
-// pitremove, the flow directions and peukerdouglas on row strips: tool 0 = pitremove (out0 = fel), 1 = d8flowdir (out0 = p int16, out1 = sd8),
-// 2 = dinfflowdir (out0 = ang, out1 = slp), 3 = peukerdouglas (out0 = ss int16); the rasters live in mappings from mgpu_alloc_shared
+// pitremove, the flow directions and peukerdouglas on row strips: tool 0 = pitremove (out[0] = fel), 1 = d8flowdir (out[0] = p int16,
+// out[1] = sd8), 2 = dinfflowdir (out[0] = ang, out[1] = slp), 3 = peukerdouglas (out[0] = ss int16); the rasters live in mappings from
+// mgpu_alloc_shared
 struct MgpuFlowJob {
   int tool = 0;
   const char* demfile = nullptr;
@@ -12,8 +13,7 @@ struct MgpuFlowJob {
   int use_mask = 0, four = 0;
   float par[3] = {0.4f, 0.1f, 0.05f};   // peukerdouglas: smoothing weights
   int nx = 0, ny = 0;
-  void* out0 = nullptr;
-  float* out1 = nullptr;
+  void* out[2] = {nullptr, nullptr};
 };
 // the sweep tools on row strips; in[] = the further inputs (NULL = not used) and out[] = the outputs (mappings from
 // mgpu_alloc_shared, nx * ny cells of the output's type) of each tool:

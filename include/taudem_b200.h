@@ -195,6 +195,22 @@ int td_d8hdisttostrm_host(const int16_t* p, const int32_t* src, float* dist, int
 int td_d8vdisttostrm_host(const int16_t* p, const float* fel, const int32_t* src, float* dist, int nx, int ny, int16_t p_nodata, int32_t src_nodata,
                           int thresh);
 long long td_disttostrm_last_levels(void);
+/* dinfdistdown: the D-infinity distance from every cell down to the stream (stream cells: src, read as int16, >= 1; no threshold,
+ * src's nodata not tested).  File level = `int dinfdistdown(char* angfile, char* felfile, char* slpfile, char* wfile, char* srcfile,
+ * char* dtsfile, int statmethod, int typemethod, int usew, int concheck)` (src/DinfDistDown.cpp:66; slp is never opened; TD_ERR_MISMATCH,
+ * after "File sizes do not match", when fel, wg or src differs from ang in size; the output takes ang's georeference).  typemethod 0 h (horizontal), 1 v (vertical: the height above the nearest
+ * drainage), 2 p (Pythagoras: sqrt(h^2 + v^2)), 3 s (surface); statmethod 0 ave, 1 max, 2 min over the cell's receivers.  Host-grid
+ * level: fel = NULL for h, w = NULL for no weights (ignored by v), dxc / dyc = ang's per-row cell sizes, used for the shares and the
+ * distances of every mode; concheck = 1: a receiver that is off the grid or nodata (or whose fel or weight is nodata) makes the cell
+ * nodata.  dd: float32, nodata MISSINGFLOAT.  Cells on a cycle of angles and every cell upslope of one keep MISSINGFLOAT.  One GPU
+ * takes a grid whose strip, (ny + 2) * td_pitch_for(nx) cells, holds fewer than 2^32 cells (TD_ERR_ARG otherwise) and whose rasters
+ * fit its memory: 15 bytes per strip cell for h, 19 for v and s, 23 for p, and 4 more with weights (27 for p with weights).
+ * Bit-exact.  td_dinfdistdown_last_levels: the levels of the last host-grid call. */
+int td_dinfdistdown(const char* angfile, const char* felfile, const char* slpfile, const char* wfile, const char* srcfile, const char* dtsfile,
+                    int statmethod, int typemethod, int usew, int concheck);
+int td_dinfdistdown_host(const float* ang, const float* fel, const float* w, const int16_t* src, float* dd, int nx, int ny, float ang_nodata,
+                         float fel_nodata, float w_nodata, const double* dxc, const double* dyc, int statmethod, int typemethod, int concheck);
+long long td_dinfdistdown_last_levels(void);
 /* flowdircond: D8-conditioned elevations.  Every cell the D8 queue of p reaches gets the smallest conditioned elevation among the
  * cells that drain into it, or its own z if that is smaller, so that elevations never rise downstream along p; the other cells keep
  * their z.  A cell whose z is nodata keeps it and still drains.  File level = `int flowdircond(char* pfile, char* zfile, char*
@@ -445,6 +461,26 @@ int td_disttostrm_seed_dev(td_ctx*, const int16_t* p, const int32_t* src, float*
                            int32_t src_nodata, void* stream);
 int td_disttostrm_levels_dev(td_ctx*, int vertical, const uint8_t* code, const float* fel, const float* rowdist, float* dist, td_strip s,
                              unsigned long long* cells, long long* levels, void* stream);
+/* dinfdistdown on a strip (dinfdistdown.cu).  td_dinfdistdown_seed_dev loads the strip's row angles from dxc / dyc (device arrays, one
+ * per owned row; td_set_halo_cell_sizes_dev gives the halo rows theirs), writes dd (and dd2, the vertical values, in the p mode; NULL
+ * otherwise) as MISSINGFLOAT and state (one byte per strip cell: the receivers, the receivers not yet evaluated, the stream bit; the
+ * strip's cells are a multiple of 4), and starts the frontier with the owned cells that wait for no receiver.  ang needs valid halo
+ * rows.  td_dinfdistdown_levels_dev runs levels until the frontier is empty: rowdist = the device table of the strip's own rows
+ * (td_slopeavedown_pass_dev's dist; unused by v), fel (v, p, s) and w (NULL: no weights) with valid halo rows; halo_out (2 pitch ints,
+ * zeroed by the caller; NULL on a strip without neighbours) counts the decrements of the donors in row 0 ([0, pitch), for the strip
+ * above) and row ny + 1 ([pitch, 2 pitch), for the strip below).  *cells / *levels as td_disttostrm_levels_dev.  On row strips the
+ * caller then hands halo_out and the first / last owned rows of dd (and dd2) to the neighbours, puts the rows it receives into the
+ * halo rows, gives the decrements it receives to td_dinfdistdown_edge_dev (dec_top for the first owned row, dec_bot for the last,
+ * NULL where there is no neighbour), which starts the next levels from the cells they release, and repeats until no strip handed a
+ * decrement over.  p mode: td_dinfdistdown_pythagoras_dev then turns dd into sqrt(dd^2 + dd2^2).  The frontier lives on the context
+ * (its listA / listB, shared with disttostrm): nothing else may run on it between the seed and the last levels call. */
+int td_dinfdistdown_seed_dev(td_ctx*, const float* ang, const int16_t* src, float* dd, float* dd2, uint8_t* state, td_strip s, float ang_nodata,
+                             const double* dxc, const double* dyc, void* stream);
+int td_dinfdistdown_levels_dev(td_ctx*, int typemethod, int statmethod, const float* ang, const float* fel, const float* w, const float* rowdist,
+                               float* dd, float* dd2, uint8_t* state, td_strip s, float fel_nodata, float w_nodata, int concheck, int* halo_out,
+                               unsigned long long* cells, long long* levels, void* stream);
+int td_dinfdistdown_edge_dev(td_ctx*, uint8_t* state, const int* dec_top, const int* dec_bot, td_strip s, void* stream);
+int td_dinfdistdown_pythagoras_dev(td_ctx*, float* dd, const float* dd2, td_strip s, void* stream);
 
 /* Peer mode (one process per GPU on one NVSwitch box): every rank exports the IPC handles of the buffers
  * its neighbours write (counts, tile scheduler, halo areas, rank 0 also the global pending counter), opens

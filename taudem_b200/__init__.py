@@ -13,12 +13,12 @@ from ._lib import (TaudemError, lib, version, device_count, launch_count, reset_
 from .api import (flood, setdird8, setdir, aread8, area,
                   pitremove_grid, d8flowdir_grid, dinfflowdir_grid, aread8_grid, areadinf_grid, contributing_areas_grid, threshold_grid, twi_grid, slopearea_grid, slopearearatio_grid, d8flowpathextremeup_grid, dinfdecayaccum_grid, dinfconclimaccum_grid, dinftranslimaccum_grid, gridnet_grid,
                   peukerdouglas_grid, lengtharea_grid, slopeavedown_grid, flowdircond_grid, retlimflow_grid,
-                  d8hdisttostrm_grid, d8vdisttostrm_grid, read_raster, write_raster, raster_info, nameadd, read_outlets)
+                  d8hdisttostrm_grid, d8vdisttostrm_grid, dinfdistdown_grid, read_raster, write_raster, raster_info, nameadd, read_outlets)
 
 __all__ = [
     "TaudemError", "lib", "version", "device_count", "launch_count", "reset_launch_count",
     "last_compute_seconds", "flood", "setdird8", "setdir", "aread8", "area", "pitremove_grid",
     "d8flowdir_grid", "dinfflowdir_grid", "aread8_grid", "areadinf_grid", "contributing_areas_grid", "threshold_grid", "twi_grid", "slopearea_grid", "slopearearatio_grid", "d8flowpathextremeup_grid", "dinfdecayaccum_grid", "dinfconclimaccum_grid", "dinftranslimaccum_grid", "gridnet_grid", "peukerdouglas_grid",
-    "lengtharea_grid", "slopeavedown_grid", "flowdircond_grid", "retlimflow_grid", "d8hdisttostrm_grid", "d8vdisttostrm_grid",
+    "lengtharea_grid", "slopeavedown_grid", "flowdircond_grid", "retlimflow_grid", "d8hdisttostrm_grid", "d8vdisttostrm_grid", "dinfdistdown_grid",
     "read_raster", "write_raster", "raster_info", "nameadd", "read_outlets",
 ]

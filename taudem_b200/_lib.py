@@ -80,6 +80,13 @@ SIGNATURES = {
     "td_disttostrm_last_levels": (C.c_longlong, []),
     "td_disttostrm_seed_dev": (_I, [_P, _P, _P, _P, _P, Strip, _I, C.c_int16, C.c_int32, _P]),
     "td_disttostrm_levels_dev": (_I, [_P, _I, _P, _P, _P, _P, Strip, _P, _P, _P]),
+    "td_dinfdistdown": (_I, [_S, _S, _S, _S, _S, _S, _I, _I, _I, _I]),
+    "td_dinfdistdown_host": (_I, [_P, _P, _P, _P, _P, _I, _I, _F, _F, _F, _P, _P, _I, _I, _I]),
+    "td_dinfdistdown_last_levels": (C.c_longlong, []),
+    "td_dinfdistdown_seed_dev": (_I, [_P, _P, _P, _P, _P, _P, Strip, _F, _P, _P, _P]),
+    "td_dinfdistdown_levels_dev": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P, Strip, _F, _F, _I, _P, _P, _P, _P]),
+    "td_dinfdistdown_edge_dev": (_I, [_P, _P, _P, _P, Strip, _P]),
+    "td_dinfdistdown_pythagoras_dev": (_I, [_P, _P, _P, Strip, _P]),
     "td_flowdircond": (_I, [_S, _S, _S]),
     "td_flowdircond_host": (_I, [_P, _P, _P, _I, _I, C.c_int16, _F]),
     "td_flowdircond_deps_dev": (_I, [_P, _P, _P, _P, Strip, C.c_int16, _P]),

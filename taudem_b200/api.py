@@ -358,6 +358,50 @@ def d8vdisttostrm_grid(p, fel, src, thresh=1, p_nodata=int(MISSINGSHORT), src_no
     return dist
 
 
+_DDD_METHODS = {"h": 0, "v": 1, "p": 2, "s": 3}
+_DDD_STATS = {"ave": 0, "max": 1, "min": 2}
+
+
+def dinfdistdown_grid(ang, src, fel=None, weights=None, method="h", stat="ave", contcheck=True, dx=30.0, dy=30.0, dxc=None, dyc=None,
+                      ang_nodata=float(MISSINGFLOAT), fel_nodata=float(FEL_NODATA), w_nodata=float(MISSINGFLOAT)):
+    """D-infinity distance down to the stream (td_dinfdistdown_host; src/DinfDistDown.cpp:66-1398): for every cell the average,
+    maximum or minimum (`stat`) over its D-infinity flow of the horizontal (`method` "h"), vertical ("v": the height above the
+    nearest drainage), Pythagoras ("p") or surface ("s") distance to the first stream cell, float32, 0 on the stream, nodata
+    MISSINGFLOAT.  Stream cells: src >= 1, src read as int16 (integers outside int16 saturate, as the reference's reader narrows
+    them).  fel: needed by v, p and s; weights: multiply the horizontal step (h, p, s).  contcheck: a receiver that is off the grid
+    or nodata (or whose fel or weight is nodata) makes the cell nodata.  dxc / dyc: ang's per-row cell sizes (default dx / dy)."""
+    if method not in _DDD_METHODS or stat not in _DDD_STATS:
+        raise ValueError(f"dinfdistdown_grid: method is one of {sorted(_DDD_METHODS)}, stat one of {sorted(_DDD_STATS)}")
+    ang = _grid(ang, np.float32)
+    s = np.asarray(src)
+    if s.dtype.kind in "iu":
+        s = np.clip(s, -32768, 32767)
+    src = _grid(s, np.int16)
+    if src.shape != ang.shape:
+        raise ValueError("dinfdistdown_grid: ang and src differ in shape")
+    if method != "h":
+        if fel is None:
+            raise ValueError(f"dinfdistdown_grid: method {method} needs fel")
+        fel = _grid(fel, np.float32)
+        if fel.shape != ang.shape:
+            raise ValueError("dinfdistdown_grid: ang and fel differ in shape")
+    else:
+        fel = None
+    if weights is not None and method != "v":
+        weights = _grid(weights, np.float32)
+        if weights.shape != ang.shape:
+            raise ValueError("dinfdistdown_grid: ang and weights differ in shape")
+    else:
+        weights = None
+    ny, nx = ang.shape
+    dxc = _rows(dx if dxc is None else dxc, ny)
+    dyc = _rows(dy if dyc is None else dyc, ny)
+    dd = np.empty((ny, nx), np.float32)
+    check(lib().td_dinfdistdown_host(_ptr(ang), _ptr(fel), _ptr(weights), _ptr(src), _ptr(dd), nx, ny, float(ang_nodata), float(fel_nodata),
+                                     float(w_nodata), _ptr(dxc), _ptr(dyc), _DDD_STATS[stat], _DDD_METHODS[method], int(bool(contcheck))))
+    return dd
+
+
 def flowdircond_grid(p, z, p_nodata=int(MISSINGSHORT), nodata=-9999.0):
     """D8-conditioned elevations (td_flowdircond_host; src/flowdircond.cpp:143-194): every cell the aread8 queue of `p` reaches gets
     the smallest conditioned elevation among the cells that drain into it, or its own z if that is smaller, so that elevations never

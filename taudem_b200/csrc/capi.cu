@@ -1081,6 +1081,106 @@ int td_d8vdisttostrm_host(const int16_t* p, const float* fel, const int32_t* src
                           int thresh) {
   return dts_host("td_d8vdisttostrm_host", true, p, fel, src, dist, nx, ny, p_nodata, src_nodata, thresh, nullptr, nullptr);
 }
+}  // extern "C"
+
+// ---- dinfdistdown (dinfdistdown.cu): Kahn's algorithm over the D-infinity receivers, one level per launch on the disttostrm frontier
+namespace {
+long long g_ddd_levels = 0;
+bool ddd_strip_ok(const td_strip& s) { return Strip(s).cells() < (1ll << 32); }
+const char* const DDD_STRIP = " (a strip holds fewer than 2^32 cells, halo rows and padding included)";
+// theta_ready: the caller has loaded the strip's row angles into ctx->theta (upload_theta_from_host)
+int ddd_seed(td_ctx* ctx, const float* ang, const int16_t* src, float* dd, float* dd2, uint8_t* state, td_strip s, float ang_nodata,
+             const double* dxc, const double* dyc, bool theta_ready, cudaStream_t st) {
+  if (int rc = check_strip(s)) return rc;
+  if (!ctx || !ang || !src || !dd || !state || (!theta_ready && (!dxc || !dyc)) || !ddd_strip_ok(s)) {
+    td::set_error(std::string("td_dinfdistdown_seed_dev: bad arguments") + DDD_STRIP);
+    return TD_ERR_ARG;
+  }
+  if (!theta_ready) { if (int rc = upload_theta(ctx, dxc, dyc, s.ny, ctx->theta, st)) return rc; }
+  td::DtsBufs b;
+  if (int rc = dts_bufs(ctx, Strip(s), &b)) return rc;
+  td::DddArgs A{};
+  A.theta = ctx->theta.as<double>();
+  A.val = dd;
+  A.val2 = dd2;
+  A.state = state;
+  return td::ddd_seed(ang, src, ang_nodata, A, Strip(s), b, st);
+}
+}  // namespace
+
+extern "C" {
+int td_dinfdistdown_seed_dev(td_ctx* ctx, const float* ang, const int16_t* src, float* dd, float* dd2, uint8_t* state, td_strip s, float ang_nodata,
+                             const double* dxc, const double* dyc, void* stream) {
+  return ddd_seed(ctx, ang, src, dd, dd2, state, s, ang_nodata, dxc, dyc, false, (cudaStream_t)stream);
+}
+int td_dinfdistdown_levels_dev(td_ctx* ctx, int typemethod, int statmethod, const float* ang, const float* fel, const float* w, const float* rowdist,
+                               float* dd, float* dd2, uint8_t* state, td_strip s, float fel_nodata, float w_nodata, int concheck, int* halo_out,
+                               unsigned long long* cells, long long* levels, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  const bool ok = ctx && ang && dd && state && typemethod >= 0 && typemethod <= 3 && statmethod >= 0 && statmethod <= 2 &&
+                  (typemethod == 1 || rowdist) && (typemethod == 0 || fel) && (typemethod != 2 || dd2) && ddd_strip_ok(s) &&
+                  (halo_out || (!s.has_top && !s.has_bot)) &&
+                  ctx->listA.cap >= sizeof(unsigned) * (size_t)Strip(s).cells();
+  if (!ok) {
+    td::set_error(std::string("td_dinfdistdown_levels_dev: bad arguments (td_dinfdistdown_seed_dev of this strip comes first, on this "
+                              "context)") + DDD_STRIP);
+    return TD_ERR_ARG;
+  }
+  td::DtsBufs b;
+  if (int rc = dts_bufs(ctx, Strip(s), &b)) return rc;
+  td::DddArgs A{ang, fel, typemethod == 1 ? nullptr : w, rowdist, ctx->theta.as<double>(), dd, typemethod == 2 ? dd2 : nullptr, state, halo_out,
+                fel_nodata, w_nodata, concheck == 1};
+  int dev = 0, sms = 1;
+  TD_CUDA(cudaGetDevice(&dev));
+  TD_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  return td::ddd_levels(typemethod, statmethod, A, Strip(s), b, sms * 4, cells, levels, (cudaStream_t)stream);
+}
+int td_dinfdistdown_edge_dev(td_ctx* ctx, uint8_t* state, const int* dec_top, const int* dec_bot, td_strip s, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  if (!ctx || !state || !ddd_strip_ok(s) || ctx->listA.cap < sizeof(unsigned) * (size_t)Strip(s).cells()) {
+    td::set_error("td_dinfdistdown_edge_dev: bad arguments (td_dinfdistdown_seed_dev of this strip comes first, on this context)");
+    return TD_ERR_ARG;
+  }
+  td::DtsBufs b;
+  if (int rc = dts_bufs(ctx, Strip(s), &b)) return rc;
+  return td::ddd_edge(state, dec_top, dec_bot, Strip(s), b, (cudaStream_t)stream);
+}
+int td_dinfdistdown_pythagoras_dev(td_ctx* ctx, float* dd, const float* dd2, td_strip s, void* stream) {
+  if (int rc = check_strip(s)) return rc;
+  if (!ctx || !dd || !dd2) {
+    td::set_error("td_dinfdistdown_pythagoras_dev: bad arguments");
+    return TD_ERR_ARG;
+  }
+  return td::ddd_pythagoras(dd, dd2, Strip(s), (cudaStream_t)stream);
+}
+long long td_dinfdistdown_last_levels(void) { return g_ddd_levels; }
+
+// src/DinfDistDown.cpp:66-90 on one strip
+int td_dinfdistdown_host(const float* ang, const float* fel, const float* w, const int16_t* src, float* dd, int nx, int ny, float ang_nodata,
+                         float fel_nodata, float w_nodata, const double* dxc, const double* dyc, int statmethod, int typemethod, int concheck) {
+  const bool ok = ang && src && dd && dxc && dyc && (typemethod == 0 || fel) && typemethod >= 0 && typemethod <= 3 && statmethod >= 0 &&
+                  statmethod <= 2;
+  return host_call("td_dinfdistdown_host", ok && (long long)(ny + 2) * td_pitch_for(nx) < (1ll << 32), nx, ny, [&](HostGrid& g) {
+    HG_TD(upload_theta_from_host(g.ctx, dxc, dyc, ny, g.ctx->theta, g.st));
+    const float* d_rd = typemethod == 1 ? nullptr : g.dist(dxc, dyc);
+    const float* d_ang = g.in(ang);
+    const float* d_fel = typemethod == 0 ? nullptr : g.in(fel);
+    const float* d_w = typemethod == 1 ? nullptr : g.in(w);
+    const int16_t* d_src = g.in(src);
+    float* d_dd = g.alloc<float>();
+    float* d_dd2 = typemethod == 2 ? g.alloc<float>() : nullptr;
+    uint8_t* d_state = g.alloc<uint8_t>();
+    g.start();
+    HG_TD(ddd_seed(g.ctx, d_ang, d_src, d_dd, d_dd2, d_state, g.s, ang_nodata, nullptr, nullptr, true, g.st));
+    long long levels = 0;
+    HG_TD(td_dinfdistdown_levels_dev(g.ctx, typemethod, statmethod, d_ang, d_fel, d_w, d_rd, d_dd, d_dd2, d_state, g.s, fel_nodata, w_nodata,
+                                     concheck, nullptr, nullptr, &levels, g.st));
+    if (typemethod == 2) HG_TD(td_dinfdistdown_pythagoras_dev(g.ctx, d_dd, d_dd2, g.s, g.st));
+    g_ddd_levels = levels;
+    g.stop();
+    g.down(dd, d_dd);
+  }, " (fewer than 2^32 strip cells)");
+}
 
 // aread8 + areadinf of one DEM in ONE call with the copies overlapped with the kernels: three streams — host -> device (p, then
 // ang), compute (aread8 as soon as p has arrived, areadinf as soon as ang has and aread8 is done), device -> host (ad8 while

@@ -1,6 +1,6 @@
 // Command line front ends: pitremove, d8flowdir, dinfflowdir, aread8, areadinf (+ the point-wise consumers threshold, twi, slopearea, slopearearatio,
-// the sibling sweep tools, the stream definitions peukerdouglas and lengtharea, slopeavedown, flowdircond, retlimflow, d8hdisttostrm and
-// d8vdisttostrm).
+// the sibling sweep tools, the stream definitions peukerdouglas and lengtharea, slopeavedown, flowdircond, retlimflow, d8hdisttostrm,
+// d8vdisttostrm and dinfdistdown).
 // Same flags, same two invocation styles and the same "print usage and exit(0)" error
 // behaviour as the reference mains (src/PitRemovemn.cpp:48-172, src/D8FlowDirmn.cpp:49-146,
 // src/DinfFlowDirmn.cpp:54-147, src/aread8mn.cpp:49-193, src/areadinfmn.cpp:49-178);
@@ -20,13 +20,25 @@ static int done() { fflush(stdout); fflush(stderr); _exit(0); return 0; }
 struct Opt {
   const char* flag;
   int kind;        // 0 = file name, 1 = switch, 2 = integer, 3 = float (ival points to a float), 4 = two floats, 5 = three floats,
-                   // 6 = double (ival points to a double)
+                   // 6 = double (ival points to a double), 7 = two method tokens (ival points to {typemethod, statmethod}: method_token)
   char* sval;      // kind 0
   int* ival;       // kind 1 (set to `set`) / kind 2 (parsed) / kind 0 (set to `set` when given, may be NULL)
   int set;
 };
 
 static void usage(const char* prog);
+
+// one token of dinfdistdown's -m (src/DinfDistDownmn.cpp:138-195): h / v / p / s set the method, ave / max / min the statistic, anything
+// else leaves both as they are
+static void method_token(const char* t, int* m) {
+  if (strcmp(t, "h") == 0) m[0] = 0;
+  else if (strcmp(t, "v") == 0) m[0] = 1;
+  else if (strcmp(t, "p") == 0) m[0] = 2;
+  else if (strcmp(t, "s") == 0) m[0] = 3;
+  if (strcmp(t, "ave") == 0) m[1] = 0;
+  else if (strcmp(t, "max") == 0) m[1] = 1;
+  else if (strcmp(t, "min") == 0) m[1] = 2;
+}
 
 // argc == 2 -> "simple usage" (nothing parsed, names derived with nameadd);
 // argc  > 2 -> flags; unknown flag or missing value -> usage, exit(0).
@@ -48,6 +60,7 @@ static void parse(int argc, char** argv, Opt* opts, int nopts) {
     else if (o->kind == 3) sscanf(argv[i], "%f", (float*)o->ival);
     else if (o->kind == 6) sscanf(argv[i], "%lf", (double*)o->ival);
     else if (o->kind == 4) { if (argc <= i + 1) usage(argv[0]); sscanf(argv[i], "%f", (float*)o->ival); i++; sscanf(argv[i], "%f", (float*)o->ival + 1); }
+    else if (o->kind == 7) { if (argc <= i + 1) usage(argv[0]); method_token(argv[i], o->ival); i++; method_token(argv[i], o->ival); }
     else if (o->kind == 5) { if (argc <= i + 2) usage(argv[0]); for (int k = 0; k < 3; ++k, ++i) sscanf(argv[i], "%f", (float*)o->ival + k); i--; }
     else sscanf(argv[i], "%d", o->ival);
     i++;
@@ -610,6 +623,54 @@ int main(int argc, char** argv) {
   if (rc == TD_ERR_MISMATCH) { fflush(stdout); _exit(5); }
   const int err = rc != 0;
   if (err) printf(DTS_V ? "D8 distance down error %d\n" : "D8 distance error %d\n", err);
+  return done();
+}
+#elif defined(TOOL_dinfdistdown)
+// src/DinfDistDownmn.cpp:50-269.  -m reads the next two tokens, each either a method or a statistic, in either order; an unknown token
+// leaves the default (ave h).  `-m x` as the last argument prints the usage here (the reference reads argv[argc] there).  -slp is
+// read and never opened.  Simple usage derives every name, -wg's included, but never uses the weights.  Rasters whose sizes differ end
+// the program with exit status 5 after "File sizes do not match", as the reference's MPI_Abort(MCW, 5) does.
+static void usage(const char* prog) {
+  printf("Simple Usage:\n %s <basefilename>\n", prog);
+  printf("Usage with specific file names:\n %s -ang <angfile>\n", prog);
+  printf("-fel <felfile> -slp <slpfile> -src <srcfile> [-wg <wfile>] -dd <dtsfile>\n");
+  printf("[-m ave h] [-nc]\n");
+  printf("<basefilename> is the name of the raw digital elevation model\n");
+  printf("<angfile> is the D-infinity flow direction input file.\n");
+  printf("<felfile> is the pit filled or carved elevation input file.\n");
+  printf("<slpfile> is the D-infinity slope input file.\n");
+  printf("<srcfile> is the stream raster input file.\n");
+  printf("<wgfile> is the D-infinity flow direction input file.\n");
+  printf("<dtsfile> is the D-infinity distance output file.\n");
+  printf("[-m ave h] is the optional method flag.\n");
+  printf("The flag -nc overrides edge contamination checking\n");
+  printf("The following are appended to the file names\n");
+  printf("before the files are opened:\n");
+  printf("ang   D-infinity contributing area file (output)\n");
+  printf("fel   pit filled or carved elevation file\n");
+  printf("slp   D-infinity slope input file file\n");
+  printf("src   Stream raster input file\n");
+  printf("wg   weight input file\n");
+  printf("dd   distance to stream output file\n");
+  exit(0);
+}
+int main(int argc, char** argv) {
+  static char ang[MAXLN], fel[MAXLN], slp[MAXLN], wfile[MAXLN], src[MAXLN], dd[MAXLN];
+  int usew = 0, concheck = 1, m[2] = {0, 0};     // {typemethod, statmethod}
+  Opt opts[] = {{"-ang", 0, ang, NULL, 0}, {"-fel", 0, fel, NULL, 0}, {"-slp", 0, slp, NULL, 0},   {"-src", 0, src, NULL, 0},
+                {"-wg", 0, wfile, &usew, 1}, {"-dd", 0, dd, NULL, 0}, {"-m", 7, NULL, m, 0},        {"-nc", 1, NULL, &concheck, 0}};
+  parse(argc, argv, opts, 8);
+  if (argc == 2) {
+    td_nameadd(ang, argv[1], "ang");
+    td_nameadd(fel, argv[1], "fel");
+    td_nameadd(slp, argv[1], "slp");
+    td_nameadd(src, argv[1], "src");
+    td_nameadd(wfile, argv[1], "wg");
+    td_nameadd(dd, argv[1], "dd");
+  }
+  const int err = td_dinfdistdown(ang, fel, slp, wfile, src, dd, m[1], m[0], usew, concheck);
+  if (err == TD_ERR_MISMATCH) { fflush(stdout); _exit(5); }
+  if (err != 0) printf("area error %d\n", err);
   return done();
 }
 #else

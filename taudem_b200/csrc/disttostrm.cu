@@ -15,45 +15,16 @@
 // code outside 1..8, or end in a cycle without a stream cell.  Pruning at values that test as nodata is exact: every cell above
 // such a value would get exactly MISSINGFLOAT, which it holds already.
 //
-// The levels run in batches without a host round trip (as k_bfs_level in flats.cu): the level bounds live in device memory,
-// the last block of level t records where level t + 1 ends, and the host reads a batch's bounds back once.
+// The levels run in batches without a host round trip (flood.cuh, shared with dinfdistdown.cu): the level bounds live in device
+// memory, the last block of level t records where level t + 1 ends, and the host reads a batch's bounds back once.
 #include "common.cuh"
 #include "ctx.h"
+#include "flood.cuh"
 #include "kernels.h"
-
-#include <vector>
 
 namespace td {
 namespace {
 constexpr int TPB = 256;
-
-// warp-aggregated append of v to list (one atomic per warp)
-__device__ __forceinline__ void dts_append(unsigned* list, unsigned long long* ctr, bool pred, unsigned v) {
-  const unsigned m = __ballot_sync(__activemask(), pred);
-  if (!pred) return;
-  const int lane = threadIdx.x & 31;
-  const int leader = __ffs(m) - 1;
-  unsigned long long base = 0;
-  if (lane == leader) base = atomicAdd(ctr, (unsigned long long)__popc(m));
-  base = __shfl_sync(m, base, leader);
-  list[base + __popc(m & ((1u << lane) - 1u))] = v;
-}
-
-// The NaN that x86 SSE arithmetic gives (the reference's, where a NaN fel travels): a NaN result carries the first NaN operand,
-// quieted, and an invalid operation on numbers (inf - inf) gives the default NaN 0xffc00000.  The GPU's own NaN result is 0x7fffffff.
-__device__ __forceinline__ float dts_quiet(float a, unsigned set) {
-  unsigned u;
-  memcpy(&u, &a, 4);
-  u |= set;
-  memcpy(&a, &u, 4);
-  return a;
-}
-__device__ __forceinline__ float dts_x86(float r, float a, float b) {
-  if (r == r) return r;
-  if (a != a) return dts_quiet(a, 0x00400000u);
-  if (b != b) return dts_quiet(b, 0x00400000u);
-  return dts_quiet(0.0f, 0xffc00000u);
-}
 
 // the value c gets from its receiver n (direction k, c's strip row r): float operations in the reference's order
 template <bool V>
@@ -119,15 +90,7 @@ __global__ void __launch_bounds__(TPB) k_dts_level(const unsigned* __restrict__ 
       dts_append(list, ctr, push, (unsigned)ci);
     }
   }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    if (atomicAdd(blkdone, 1u) == gridDim.x - 1) {          // the last block: every append of this level is done
-      __threadfence();
-      bounds[t + 1] = *reinterpret_cast<volatile unsigned long long*>(ctr);
-      *blkdone = 0;
-    }
-  }
+  flood_level_done(bounds, t, ctr, blkdone);
 }
 
 // blockIdx.y = 0: the first owned row, 1: the last (the same row of a one-row strip is taken once)
@@ -177,40 +140,10 @@ int dts_levels(bool vertical, const unsigned char* code, const float* fel, const
     TD_LAUNCHED();
     TD_CUDA(cudaGetLastError());
   }
-  // where the frontier stands: [consumed, appended)
-  unsigned long long hc[2] = {0, 0};
-  std::vector<unsigned long long> hb(DTS_BATCH);
-  TD_CUDA(cudaMemcpyAsync(hc, b.ctr, sizeof hc, cudaMemcpyDeviceToHost, st));
-  TD_CUDA(cudaStreamSynchronize(st));
-  const unsigned long long start = hc[1];
-  unsigned long long lo = start, hi = hc[0];
-  long long nlev = 0;
-  while (hi > lo) {
-    // bounds[0, 1] = the frontier; levels 1..DTS_BATCH write bounds[2 .. DTS_BATCH + 1]
-    TD_CUDA(cudaMemcpyAsync(b.bounds, b.ctr + 1, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
-    TD_CUDA(cudaMemcpyAsync(b.bounds + 1, b.ctr, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
-    for (int t = 1; t <= DTS_BATCH; ++t) {
-      if (vertical) k_dts_level<true><<<grid, TPB, 0, st>>>(b.list, b.bounds, t, code, fel, dist, val, s, b.list, b.ctr, b.blkdone);
-      else k_dts_level<false><<<grid, TPB, 0, st>>>(b.list, b.bounds, t, code, fel, dist, val, s, b.list, b.ctr, b.blkdone);
-      TD_LAUNCHED();
-    }
-    TD_CUDA(cudaGetLastError());
-    TD_CUDA(cudaMemcpyAsync(hb.data(), b.bounds + 2, sizeof(unsigned long long) * DTS_BATCH, cudaMemcpyDeviceToHost, st));
-    TD_CUDA(cudaMemcpyAsync(b.ctr + 1, b.bounds + DTS_BATCH, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));   // consumed
-    TD_CUDA(cudaStreamSynchronize(st));
-    unsigned long long prev = hi;
-    ++nlev;                                                     // level 1 of the batch had cells
-    for (int j = 0; j < DTS_BATCH; ++j) {
-      if (hb[j] == prev) break;                          // level j + 2 is empty
-      if (j + 1 < DTS_BATCH) ++nlev;
-      prev = hb[j];
-    }
-    lo = DTS_BATCH >= 2 ? hb[DTS_BATCH - 2] : hi;        // the frontier after the batch: [bounds[B], bounds[B + 1])
-    hi = hb[DTS_BATCH - 1];
-  }
-  if (cells) *cells = hi - start;
-  if (levels) *levels = nlev;
-  return TD_OK;
+  return flood_levels(b, [&](int t) {
+    if (vertical) k_dts_level<true><<<grid, TPB, 0, st>>>(b.list, b.bounds, t, code, fel, dist, val, s, b.list, b.ctr, b.blkdone);
+    else k_dts_level<false><<<grid, TPB, 0, st>>>(b.list, b.bounds, t, code, fel, dist, val, s, b.list, b.ctr, b.blkdone);
+  }, cells, levels, st);
 }
 
 }  // namespace td

@@ -71,6 +71,23 @@ int dts_seed(const short* p, const int* src, float* val, unsigned char* code, co
 // blocks per level); *cells = the list entries added since the last call (with the seeds), *levels = the non-empty levels run
 int dts_levels(bool vertical, const unsigned char* code, const float* fel, const float* dist, float* val, const Strip& s, const DtsBufs& b, int grid,
                unsigned long long* cells, long long* levels, cudaStream_t st);
+// dinfdistdown.cu: Kahn's algorithm over the D-infinity receivers, one level per launch on the same frontier machinery (flood.cuh).
+// theta: the strip's per-row angle table (theta_of_row); dist: the cell-to-cell distances of the owned rows (8 per row); val2: the
+// vertical values of the p mode (else NULL); state: one byte per strip cell, the strip's size a multiple of 4 bytes; halo_out: the
+// decrements of the donors in the halo rows, [0, pitch) row 0 (sent up), [pitch, 2 pitch) row ny + 1 (sent down); NULL on one strip.
+struct DddArgs {
+  const float* ang; const float* fel; const float* w; const float* dist; const double* theta;
+  float* val; float* val2; unsigned char* state; int* halo_out;
+  float fel_nodata, w_nodata;
+  int concheck;
+};
+int ddd_seed(const float* ang, const short* src, float ang_nodata, const DddArgs& A, const Strip& s, const DtsBufs& b, cudaStream_t st);
+// mode 0..3 = h, v, p, s; stat 0..2 = ave, max, min
+int ddd_levels(int mode, int stat, const DddArgs& A, const Strip& s, const DtsBufs& b, int grid, unsigned long long* cells, long long* levels,
+               cudaStream_t st);
+// the decrements received for the first / last owned row (NULL: no neighbour there); the released cells join the frontier
+int ddd_edge(unsigned char* state, const int* dec_top, const int* dec_bot, const Strip& s, const DtsBufs& b, cudaStream_t st);
+int ddd_pythagoras(float* h, const float* v, const Strip& s, cudaStream_t st);
 int launch_mask_ok(const int* mask, float* ok, const Strip& s, int thresh, cudaStream_t st);
 int launch_gord_finish(const float* g, const short* p, const float* ok, const unsigned short* node, short* gord, const Strip& s, short p_nodata,
                        int outlets, cudaStream_t st);

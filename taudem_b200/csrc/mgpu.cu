@@ -144,19 +144,18 @@ void peer_sweep(Shared* S, int world, td_ctx* ctx, const td_strip& s, cudaStream
   run();
   MG_BAR();
 }
-// one sweep in rounds (after the deps call): evaluate until no cell of the strip is ready, hand the decrement counts and the edge
-// rows of the travelling value (val; val2 = a second one, or NULL) to the neighbours, repeat until nobody handed anything over.
-// Returns the rounds.
-template <class Run>
-int sweep_rounds(Shared* S, char* extra, int rank, int world, const td_strip& s, td_ctx* ctx, cudaStream_t st, int* d_halo, float* val, float* val2,
-                 Run&& run) {
+// rounds of a downslope or upslope evaluation on row strips (after the caller has started it): run() evaluates until no cell of the
+// strip is ready, writing the decrement counts it hands over into d_halo; they and the edge rows of the travelling value (val; val2 =
+// a second one, or NULL) go to the neighbours; apply(dec_top, dec_bot) takes the counts received for the first / last owned row (NULL
+// where there is no neighbour); repeat until nobody handed anything over.  Returns the rounds.
+template <class Run, class Apply>
+int exchange_rounds(Shared* S, char* extra, int rank, int world, const td_strip& s, int* d_halo, float* val, float* val2, Run&& run, Apply&& apply) {
   const int ny = s.ny;
   const RoundBuf R{extra, s.pitch};
   std::vector<int> hal(2 * (size_t)s.pitch), dec(2 * (size_t)s.pitch);
   float* vals[2] = {val, val2};
   const int nv = val2 ? 2 : 1;
   int rounds = 0;
-  MG_TD(td_sweep_begin_dev(ctx, s, st));
   for (;;) {
     run();
     ++rounds;
@@ -187,8 +186,7 @@ int sweep_rounds(Shared* S, char* extra, int rank, int world, const td_strip& s,
     MG_BAR();
     if (all == 0) break;                                      // ringTerm: nobody handed anything over
     MG_CUDA(cudaMemcpy(d_halo + 2 * (size_t)s.pitch, dec.data(), sizeof(int) * 2 * (size_t)s.pitch, cudaMemcpyHostToDevice));
-    MG_TD(td_sweep_apply_halo_dev(ctx, s, rank > 0 ? d_halo + 2 * (size_t)s.pitch : nullptr,
-                                  rank < world - 1 ? d_halo + 3 * (size_t)s.pitch : nullptr, st));
+    apply(rank > 0 ? d_halo + 2 * (size_t)s.pitch : nullptr, rank < world - 1 ? d_halo + 3 * (size_t)s.pitch : nullptr);
   }
   return rounds;
 }
@@ -210,6 +208,7 @@ const SibTool sib_tools[MgpuSibJob::NTOOLS] = {
     {true, {F32, F32, F32}},             // AREADINF
     {false, {tdio::DT_I32, F32, F32}},   // D8HDIST
     {false, {tdio::DT_I32, F32, F32}},   // D8VDIST
+    {true, {tdio::DT_I16, F32, F32}},    // DINFDISTDOWN
 };
 
 void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int world) {
@@ -259,7 +258,8 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
   }
   std::vector<double> dxc, dyc;
   in.cell_sizes(&dxc, &dyc);
-  if (J.tool == MgpuSibJob::GRIDNET || J.tool == MgpuSibJob::SLOPEAVEDOWN || J.tool == MgpuSibJob::D8HDIST) {
+  if (J.tool == MgpuSibJob::GRIDNET || J.tool == MgpuSibJob::SLOPEAVEDOWN || J.tool == MgpuSibJob::D8HDIST ||
+      (J.tool == MgpuSibJob::DINFDISTDOWN && J.typemethod != 1)) {
     if (J.tool == MgpuSibJob::GRIDNET) {
       if (J.in[0]) MG_CUDA(cudaMalloc(&d_ok, cells * 4));
       MG_CUDA(cudaMalloc(&d_g, cells * 2));
@@ -294,7 +294,11 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
       MG_CUDA(cudaStreamSynchronize(st));
     };
     if (peer) { peer_sweep(S, world, ctx, s, st, run); rounds += 1; }
-    else rounds += sweep_rounds(S, extra, rank, world, s, ctx, st, d_halo, d_val, val2, run);
+    else {
+      MG_TD(td_sweep_begin_dev(ctx, s, st));
+      rounds += exchange_rounds(S, extra, rank, world, s, d_halo, d_val, val2, run,
+                                [&](const int* top, const int* bot) { MG_TD(td_sweep_apply_halo_dev(ctx, s, top, bot, st)); });
+    }
   };
   // rows 1..ny of a strip array -> this rank's rows of an output mapping
   auto store = [&](void* out, const void* d, size_t eb) {
@@ -399,6 +403,28 @@ void sibling_worker(const MgpuSibJob& J, Shared* S, char* extra, int rank, int w
         MG_BAR();
         if (any == 0) break;                                  // nobody added a cell: every edge row is final
       }
+      break;
+    }
+    case MgpuSibJob::DINFDISTDOWN: {
+      // the reference's ring loop (src/DinfDistDown.cpp:243-357): levels until the strip's frontier is empty, the decrements of the
+      // donors in the halo rows (neighbor->addBorders()) and the value raster's edge rows (dts->share(); two rasters in the p mode) to
+      // the neighbours, the received decrements start the next levels; until nobody handed a decrement over (ringTerm)
+      const bool p_mode = J.typemethod == 2;
+      float* d_v = nullptr;                                   // the p mode's vertical values
+      MG_CUDA(cudaMalloc(&d_code, cells));
+      if (p_mode) MG_CUDA(cudaMalloc(&d_v, cells * 4));
+      MG_TD(td_dinfdistdown_seed_dev(ctx, ang, (const int16_t*)d_in[0], d_val, d_v, d_code, s, a_nd, d_dx, d_dx + ny, st));
+      auto run = [&]() {
+        MG_CUDA(cudaMemsetAsync(d_halo, 0, sizeof(int) * 2 * (size_t)s.pitch, st));
+        MG_TD(td_dinfdistdown_levels_dev(ctx, J.typemethod, J.statmethod, ang, f1, f2, d_dist, d_val, d_v, d_code, s, nd[1], nd[2], J.contcheck, d_halo,
+                                         nullptr, nullptr, st));
+        MG_CUDA(cudaStreamSynchronize(st));
+      };
+      rounds += exchange_rounds(S, extra, rank, world, s, d_halo, d_val, d_v, run,
+                                [&](const int* top, const int* bot) { MG_TD(td_dinfdistdown_edge_dev(ctx, d_code, top, bot, s, st)); });
+      if (p_mode) MG_TD(td_dinfdistdown_pythagoras_dev(ctx, d_val, d_v, s, st));
+      MG_CUDA(cudaStreamSynchronize(st));
+      cudaFree(d_v);
       break;
     }
     case MgpuSibJob::TRANSLIM:

@@ -29,14 +29,17 @@ struct MgpuFlowJob {
 //   AREADINF      areadinf          in: w (or NULL)        out: sca
 //   D8HDIST       d8hdisttostrm     in: src (int32)        out: dist (thresh)
 //   D8VDIST       d8vdisttostrm     in: src (int32), fel   out: dist (thresh)
+//   DINFDISTDOWN  dinfdistdown      in: src (int16), fel (or NULL), w (or NULL)   out: dd (typemethod, statmethod, contcheck)
 struct MgpuSibJob {
-  enum { EXTREMEUP = 0, GRIDNET, DECAY, CONCLIM, TRANSLIM, SLOPEAVEDOWN, FLOWDIRCOND, RETLIMFLOW, AREAD8, AREADINF, D8HDIST, D8VDIST, NTOOLS };
+  enum { EXTREMEUP = 0, GRIDNET, DECAY, CONCLIM, TRANSLIM, SLOPEAVEDOWN, FLOWDIRCOND, RETLIMFLOW, AREAD8, AREADINF, D8HDIST, D8VDIST, DINFDISTDOWN,
+         NTOOLS };
   int tool = EXTREMEUP;
   const char* dirfile = nullptr;              // p (D8 tools) or ang
   const char* in[3] = {nullptr, nullptr, nullptr};
   int usemax = 1, contcheck = 1, thresh = 0;   // thresh: gridnet, d8hdisttostrm, d8vdisttostrm
   float csol = 0.f;
   double dn = 0.; int niter = 0;              // slopeavedown
+  int typemethod = 0, statmethod = 0;         // dinfdistdown
   int nx = 0, ny = 0;
   void* out[3] = {nullptr, nullptr, nullptr};
 };

@@ -686,4 +686,29 @@ int td_d8vdistdown(const char* pfile, const char* felfile, const char* srcfile, 
   return disttostrm(true, pfile, felfile, srcfile, distfile, thresh);
 }
 
+// src/DinfDistDown.cpp:66-1398: ang (float), fel (float; v, p and s), wg (float; h, p and s with usew) and src (read as int16) in, opened
+// in the reference's order (h: ang, wg, src; v: ang, fel, src; p and s: ang, fel, wg, src; slp is never opened), dd out (float32, nodata
+// MISSINGFLOAT, the georeference of ang).  The shares and distances use ang's per-row cell sizes.
+int td_dinfdistdown(const char* angfile, const char* felfile, const char* slpfile, const char* wfile, const char* srcfile, const char* dtsfile,
+                    int statmethod, int typemethod, int usew, int concheck) {
+  (void)slpfile;
+  return guarded([&] {
+    static const char* const banner[4] = {"DinfDistDown -h", "DinfDistDown -v", "DinfDistDown -p", "DinfDistDown -s"};
+    if (typemethod < 0 || typemethod > 3 || statmethod < 0 || statmethod > 2) { td::set_error("td_dinfdistdown: bad method"); return TD_ERR_ARG; }
+    const bool uf = typemethod != 0, uw = usew == 1 && typemethod != 1;
+    td::MgpuSibJob J;
+    J.tool = td::MgpuSibJob::DINFDISTDOWN; J.dirfile = angfile; J.in[0] = srcfile; J.in[1] = uf ? felfile : nullptr; J.in[2] = uw ? wfile : nullptr;
+    J.typemethod = typemethod; J.statmethod = statmethod; J.contcheck = concheck;
+    Tool t{banner[typemethod], "DinfDistDown",
+           {{angfile, F32}, {felfile, F32, "elevation grid does not match", SIZES, uf}, {wfile, F32, "weight grid does not match", SIZES, uw},
+            {srcfile, I16, "stream raster does not match"}},
+           {{0, dtsfile, F32, MISSINGFLOAT}}, SWEEP, "Processors", nullptr, &J};
+    return run(t, [&](const Grids& g) {
+      const Input &a = g.in[0], &z = g.in[1], &w = g.in[2], &s = g.in[3];
+      return td_dinfdistdown_host(a.as<float>(), uf ? z.as<float>() : nullptr, uw ? w.as<float>() : nullptr, s.as<int16_t>(), g.out<float>(0), a.nx, a.ny,
+                                  a.fnd(), uf ? z.fnd() : 0.f, uw ? w.fnd() : 0.f, a.dxc.data(), a.dyc.data(), statmethod, typemethod, concheck);
+    });
+  });
+}
+
 }  // extern "C"
